@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- OF-3B training tokens/sec on B200 (BASELINE.json metric), one process per GPU.
+"""bench.py -- OF-3B training tokens/sec on H100 (BASELINE.json metric), one process per GPU.
 
     python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo's CUDA path
     python bench.py --impl reference [--steps K] [--warmup W]      # CPU port of the reference (oracle), host cores
+    python bench.py ... --dump-outputs DIR                          # also save what the last timed step computed
 
 Workload (BASELINE.json configs[1], SURVEY.md C2): OF-3B = ViT-L/14 + MPT-1B-shaped LM (HF MptForCausalLM,
 random init -- there is no network for checkpoints) with a gated cross-attention block before every decoder
@@ -42,6 +43,9 @@ def parse_args():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--gemm-shapes", default=None, help="write the per-shape GEMM table of the instrumented pass here")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last one computed (loss; seeded samples of the updated "
+                         "trainable parameters and of their gradients) as DIR/<name>.npy, so two builds can be compared")
     ap.add_argument("--batch", type=int, default=32)
     ap.add_argument("--t_img", type=int, default=2)
     ap.add_argument("--t_txt", type=int, default=256)
@@ -126,8 +130,17 @@ class ClockSampler:
 
 
 # ----------------------------------------------------------------------------------------------- GEMM timing hook
+def gemm_tiles(m, n, splits):
+    """Work items of the persistent GEMM grid: 128 x 128 output tiles times split-K slices."""
+    return ((m + 127) // 128) * ((n + 127) // 128) * splits
+
+
+def num_sms():
+    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+
+
 class GemmTimer:
-    """CUDA-event timing of every tcgen05 GEMM launch inside the timed region (events are recorded on the stream
+    """CUDA-event timing of every GEMM launch inside the timed region (events are recorded on the stream
     the kernel is launched on; the overhead is two event records per launch)."""
 
     def __init__(self):
@@ -162,17 +175,17 @@ class GemmTimer:
             setattr(self._mod, name, fn)
 
     def by_shape(self, steps):
-        """Per (variant, M, N, K, splits): launches/step, mean us, TFLOP/s, tiles and waves of the 2-CTA 256x256 grid."""
+        """Per (variant, M, N, K, splits): launches/step, mean us, TFLOP/s, 128 x 128 tiles and waves over the SMs."""
         acc = {}
         for e0, e1, flop, epi, a_mn, b_mn, shape in self.records:
             d = acc.setdefault((epi, a_mn, b_mn) + shape, [0.0, 0.0, 0])
             d[0] += e0.elapsed_time(e1); d[1] += flop; d[2] += 1
         rows = []
         for (epi, a_mn, b_mn, m, n, k, splits), (ms, flop, cnt) in acc.items():
-            tiles = ((m + 255) // 256) * ((n + 255) // 256) * splits
+            tiles = gemm_tiles(m, n, splits)
             rows.append({"epi": epi, "a_mn": a_mn, "b_mn": b_mn, "M": m, "N": n, "K": k, "splits": splits,
                          "launches_per_step": cnt / steps, "ms_per_step": ms / steps, "us_per_launch": 1e3 * ms / cnt,
-                         "TFLOP/s": flop / (ms * 1e-3) / 1e12 if ms else 0.0, "tiles": tiles, "waves_74": tiles / 74.0})
+                         "TFLOP/s": flop / (ms * 1e-3) / 1e12 if ms else 0.0, "tiles": tiles, "waves": tiles / num_sms()})
         return sorted(rows, key=lambda r: -r["ms_per_step"])
 
     def summary(self):
@@ -190,7 +203,7 @@ class GemmTimer:
 
 class GraphGemmTimer:
     """Per-GEMM device times INSIDE a captured CUDA graph of the training step: an event-record node with the
-    cudaEventRecordExternal flag before and after every tcgen05 GEMM launch (cudart called directly on the capturing
+    cudaEventRecordExternal flag before and after every GEMM launch (cudart called directly on the capturing
     stream; torch.cuda.Event cannot be recorded during capture).  Inside a graph there is no CPU between the nodes, so
     the pairs bracket exactly the kernel (plus one node-to-node gap), unlike event pairs in an eager pass, which also
     contain whatever time the host needs to enqueue the launch when the step is CPU-bound."""
@@ -394,6 +407,34 @@ def run_reference(args):
 
 
 # ----------------------------------------------------------------------------------------------- our arm
+DUMP_SAMPLE = 1 << 22     # elements per sampled array: 16 MB in float32, 32 MB for the whole dump
+
+
+def dump_outputs(out_dir, loss, trainer):
+    """What the last timed step computed, as float32/float64 .npy files: the loss it returned, and the trainable
+    parameters it updated and their gradients, both sampled at the same flat positions (a fixed seed draws them, so
+    every run and every build samples the same elements)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    params, grads = trainer.bucket.params, trainer.bucket.grads
+    n = params.numel()
+    idx = torch.randint(0, n, (min(n, DUMP_SAMPLE),), generator=torch.Generator().manual_seed(1234)).sort().values
+    idx_dev = idx.to(params.device)
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray(float(loss.detach().float().item()), dtype=np.float64))
+    np.save(os.path.join(out_dir, "params_sample.npy"), params[idx_dev].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "grads_sample.npy"), grads[idx_dev].float().cpu().numpy())
+
+
+def gpu_identity(index):
+    """Card name and power limit: part of every number this run reports."""
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit,clocks.max.sm",
+                            "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
+        return r.stdout.strip() or None
+    except Exception:
+        return None
+
+
 def run_ours(args):
     import torch.distributed as dist
     from open_flamingo_b200 import _lib, ops
@@ -501,8 +542,15 @@ def run_ours(args):
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
-    ms_total = timed(lambda: run_step(resident), args.steps)
+    last = {}
+
+    def timed_step():
+        last["loss"] = run_step(resident)
+
+    ms_total = timed(timed_step, args.steps)
     clocks = sampler.stop() if rank == 0 else {}
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["loss"], trainer)
     ms_step = ms_total / args.steps
     tokens = world * B * T_txt * MB
     # host time needed to ENQUEUE one step (no sync inside): must stay well below ms_step or the GPU starves
@@ -512,7 +560,7 @@ def run_ours(args):
     cpu_enqueue_ms = (time.perf_counter() - t_cpu0) * 1e3
     torch.cuda.synchronize()
 
-    # ---- same K steps again with a CUDA-event pair around every tcgen05 GEMM launch (roofline numerator/denominator)
+    # ---- same K steps again with a CUDA-event pair around every GEMM launch (roofline numerator/denominator)
     timer = GemmTimer()
     timer.wrap(ops)
     ms_instr = timed(lambda: train_step(resident), args.steps)
@@ -554,10 +602,10 @@ def run_ours(args):
                 d2[0] += ms_; d2[1] += flop; d2[2] += 1
             shape_rows = []
             for (epi, a_mn, b_mn, m, n, k, splits), (ms_, flop, cnt) in acc.items():
-                tiles = ((m + 255) // 256) * ((n + 255) // 256) * splits
+                tiles = gemm_tiles(m, n, splits)
                 shape_rows.append({"epi": epi, "a_mn": a_mn, "b_mn": b_mn, "M": m, "N": n, "K": k, "splits": splits,
                                    "launches_per_step": cnt, "ms_per_step": ms_, "us_per_launch": 1e3 * ms_ / cnt,
-                                   "TFLOP/s": flop / (ms_ * 1e-3) / 1e12 if ms_ else 0.0, "tiles": tiles, "waves_74": tiles / 74.0})
+                                   "TFLOP/s": flop / (ms_ * 1e-3) / 1e12 if ms_ else 0.0, "tiles": tiles, "waves": tiles / num_sms()})
             shape_rows.sort(key=lambda r: -r["ms_per_step"])
             gemm_method = ("cudaEventRecordExternal node pair around every GEMM launch INSIDE a captured CUDA graph of the step, "
                            f"mean of {args.steps} replays")
@@ -583,26 +631,12 @@ def run_ours(args):
     ms_e2e = timed(e2e_step, args.steps) / args.steps
 
     if rank == 0:
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except Exception:
-            pass
-        peak_tf = peaks.get("bf16_tflops_sustained") or 1400.0
-        peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)" if peaks else \
-            "fallback 1.4 PF sustained (B200_PROFILING.md)"
+        peak_tf = 989.0
+        peak_src = "NVIDIA data sheet, H100 SXM dense BF16 at 700 W (a peak, not a measured rate)"
         achieved_tf = gemm_flop / (gemm_ms * 1e-3) / 1e12 if gemm_ms > 0 else 0.0
-        traffic = None
-        try:  # mean DRAM bytes per launch of the FFN GEMMs from the committed `ncu --set full` capture
-            tj = json.load(open(os.path.join(ROOT, "profiles", "gemm_traffic.json")))
-            traffic = tj.get("mean_dram_bytes_per_launch")
-        except Exception:
-            pass
-        roofline = {"bound": "tensor", "kernel": "ofk::gemm2_kernel<A_MN,B_MN,EPI> / gemm_kernel<BN,...> (tcgen05 cta_group::2 / ::1, every launch in the timed region)",
+        roofline = {"bound": "tensor", "kernel": "ofk::gemm_kernel<A_MN,B_MN,EPI> (wgmma + TMA, every launch in the timed region)",
                     "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved_tf / peak_tf,
-                    "peak_source": peak_src, "traffic": traffic,
-                    "traffic_source": "STATIC: mean dram__bytes_read+write per launch of the FFN GEMMs in the committed ncu --set full "
-                                      "capture profiles/gemm_traffic.json (see its `build` field), not re-measured by this run",
+                    "peak_source": peak_src,
                     "launches_per_step": gemm_n / gemm_steps, "gemm_ms_per_step": gemm_ms / gemm_steps,
                     "share_of_step": (gemm_ms / gemm_steps) / ms_step if ms_step else None,
                     "method": gemm_method,
@@ -632,11 +666,12 @@ def run_ours(args):
                 "config": {"workload": f"{args.model.upper()} (ViT-L/14 + {LM_NAME.get(args.model, 'tiny')}-shaped HF MptForCausalLM, xattn_every={every}) "
                                        "amp_bf16 train step: fwd+bwd+grad all-reduce+clip+AdamW",
                            "global_batch": world * B * MB, "per_gpu_batch": B, "micro_batches": MB, "t_img": T_img, "seq_len": T_txt,
-                           "parallelism": f"dp{world}", "frozen_lm_blocks": args.lm, "cuda_graph": graph_used, "l2": "per-step working set (>10 GB weights+activations) exceeds the 126 MB L2; no explicit flush",
+                           "parallelism": f"dp{world}", "frozen_lm_blocks": args.lm, "cuda_graph": graph_used, "l2": "per-step working set (>10 GB weights+activations) exceeds the 50 MB L2; no explicit flush",
                            "trainable_params": sum(p.numel() for p in model.parameters() if p.requires_grad)},
                 "e2e": {"value": tokens / (ms_e2e * 1e-3), "unit": UNIT, "ms_per_step": ms_e2e,
                         "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": 4},
                 "gpu_launches": launches, "cpu_enqueue_ms_per_step": cpu_enqueue_ms, "clocks": clocks,
+                "gpu": gpu_identity(local_rank),
                 "roofline": roofline}
         if cpu_baseline is not None:
             line["cpu_baseline"] = cpu_baseline

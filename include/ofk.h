@@ -1,5 +1,5 @@
 /*
- * ofk.h -- C ABI of libofk.so: the B200 (sm_100a) kernels behind the OpenFlamingo dense hot path.
+ * ofk.h -- C ABI of libofk.so: the H100 (sm_90a) kernels behind the OpenFlamingo dense hot path.
  *
  * The reference (mlfoundations/open_flamingo) is pure eager PyTorch and has NO native interface; each
  * entry point below names the reference Python it replaces (paths relative to the reference repo root,
@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define OFK_ABI_VERSION 2
+#define OFK_ABI_VERSION 3
 
 enum {
   OFK_OK = 0,
@@ -33,7 +33,7 @@ enum {
   OFK_ERR_DRIVER = -4  /* driver entry point (tensor-map encode) unavailable or failed */
 };
 
-/* GEMM epilogues (fused into the tcgen05 kernel's TMEM->global stage). */
+/* GEMM epilogues (fused into the wgmma kernel's register->global stage). */
 enum {
   OFK_EPI_STORE_BF16 = 0,      /* out(bf16) = acc                                            nn.Linear, helpers.py:35-37,153-155 */
   OFK_EPI_STORE_F32 = 1,       /* out(f32)  = acc                                                                               */
@@ -54,13 +54,14 @@ int ofk_abi_version(void);
 long long ofk_launch_count(void);
 
 /* ------------------------------------------------------------------------------------------------
- * GEMM  out[m,n] = epi( sum_k A(m,k) * B(n,k) ), bf16 operands, fp32 accumulate in TMEM (tcgen05).
+ * GEMM  out[m,n] = epi( sum_k A(m,k) * B(n,k) ), bf16 operands, fp32 accumulate in registers (wgmma).
  *   a_mn_major = 0: A stored [M,K] (K contiguous).  = 1: A stored [K,M] (M contiguous).
  *   b_mn_major = 0: B stored [N,K] (K contiguous).  = 1: B stored [K,N] (N contiguous).
  *   forward  y = x W^T       : A=x [R,in]  (0), B=W [out,in] (0)         nn.Linear (helpers.py:18-21,35-37,153-155)
  *   dgrad    dx = dy W       : A=dy [R,out](0), B=W [out,in] (1), K=out  autograd of the above
  *   wgrad    dW += dy^T x    : A=dy [R,out](1), B=x [R,in]   (1), K=R    autograd of the above (ATOMIC_F32)
- *   splits  : split-K factor (ATOMIC_F32 only).  block_n: 0 = auto, else 128 or 256.
+ *   splits  : split-K factor (ATOMIC_F32 only).  block_n: 0, 128, 256 or 512 -- a tile-width hint; the sm_90a
+ *             kernel always uses 128 x 128 tiles, so every accepted value gives the same result.
  * Requirements: N % 16 == 0; operand base pointers 16-byte aligned, lda/ldb % 8 == 0.
  */
 int ofk_gemm_bf16(int epi, int a_mn_major, int b_mn_major, const void* A, long long lda, const void* B,
@@ -68,23 +69,9 @@ int ofk_gemm_bf16(int epi, int a_mn_major, int b_mn_major, const void* A, long l
                   void* out2, long long ldo2, const void* aux, long long ldaux, const float* bias,
                   const float* gate, void* stream);
 
-/* Same GEMM with a caller-owned scratch buffer that enables the "tail split": when the last round of the persistent
- * 256 x 256-tile grid would be at most half full (e.g. the N = 2048 projections of MPT-1B: 256 tiles on 74 SM pairs =
- * 3.46 rounds), its tiles are cut into 2-4 k-slices that run on the otherwise idle SM pairs; the slices exchange fp32
- * partial accumulators through `workspace` (L2-resident) and the last slice applies the fused epilogue, so results
- * do not depend on whether the split is taken beyond fp32 summation order.  `workspace` must hold at least
- * ofk_gemm_workspace_bytes() bytes, be 16-byte aligned, have its first 16384 bytes zeroed once before first use, and
- * must not be shared by GEMMs that may run concurrently (one buffer per stream).  NULL = plain ofk_gemm_bf16.
- * Replaces the same reference lines as ofk_gemm_bf16. */
-long long ofk_gemm_workspace_bytes(void);
-int ofk_gemm_bf16_ws(int epi, int a_mn_major, int b_mn_major, const void* A, long long lda, const void* B,
-                     long long ldb, int M, int N, int K, int splits, int block_n, void* out, long long ldo,
-                     void* out2, long long ldo2, const void* aux, long long ldaux, const float* bias,
-                     const float* gate, void* workspace, long long workspace_bytes, void* stream);
-
-/* Leave `n` SMs (rounded down to whole pairs, at most 64) out of every persistent GEMM grid launched from now on; returns
- * the previous value.  The data-parallel step uses it while gradient-chunk all-reduces are in flight (train.GradBucket):
- * a persistent grid that owns all 148 SMs lets NCCL's CTAs in only at kernel boundaries, which serialises the
+/* Leave `n` SMs (rounded down to whole TPCs of two SMs, at most 64) out of every persistent GEMM grid launched from now
+ * on; returns the previous value.  The data-parallel step uses it while gradient-chunk all-reduces are in flight
+ * (train.GradBucket): a persistent grid that owns all 132 SMs lets NCCL's CTAs in only at kernel boundaries, which serialises the
  * "overlapped" reduction behind each GEMM.  0 restores the full grid. */
 int ofk_gemm_reserve_sms(int n);
 
@@ -124,11 +111,9 @@ int ofk_layernorm_bwd(const void* dy, int dy_is_f32, long long lddy, int rows_pe
 
 /* ------------------------------------------------------------------------------------------------
  * Attention core  O = softmax(scale * Q K^T + mask) V  per (batch, head), head_dim = 64, bf16 in/out,
- * fp32 softmax, online (flash-style).
- * Default implementation (csrc/attention_tc.cu): Q/K/V (and dO) tiles staged by TMA (cp.async.bulk.tensor, 128-byte
- * swizzle), QK^T / PV and the five backward contractions as tcgen05.mma with TMEM accumulators, lane-per-row softmax
- * on the TMEM read-out, P / dS through swizzled shared memory.  It needs batch strides == rows * row stride and
- * 16-byte aligned bases; any other layout runs the mma.sync kernels of csrc/attention.cu (same results).
+ * fp32 softmax, online (flash-style).  Default: warpgroup kernels whose QK^T / PV (and the backward's five products) are
+ * wgmma on 128-byte-swizzled shared-memory tiles, P / dS fed from registers; the mma.sync kernels of the same files are
+ * the A/B reference (ofk_attn_force_legacy).
  *   q: [batch, nq, heads*64] (ldq row stride), k/v: [batch, nk, heads*64] (ldk/ldv), o like q (ldo).
  *   q_bstride/k_bstride...: batch strides in elements.  lse: [batch, heads, nq] f32 (log2 domain, for bwd).
  *   mask_mode: 0 = none                                              PerceiverAttention helpers.py:58-63, ViT MHA
@@ -143,11 +128,6 @@ int ofk_attn_fwd(const void* q, const void* k, const void* v, void* o, float* ls
                  long long v_bstride, long long ldv, long long o_bstride, long long ldo, float scale,
                  int mask_mode, const int* text_time, int keys_per_media, void* stream);
 
-/* Scratch the tensor-core backward needs: an fp32 dQ accumulator [batch*nq, heads*head_dim] whenever more than one
- * 128-key tile contributes to a query row (0 bytes when nk <= 128).  Caller-owned, 16-byte aligned, need not be
- * initialised.  Without it (NULL / too small) the backward runs the mma.sync kernels. */
-long long ofk_attn_bwd_workspace_bytes(int batch, int heads, int head_dim, int nq, int nk);
-
 /* Backward of the above.  delta: [batch, heads, nq] f32 scratch.  dq like q; dk/dv like k/v (bf16).
  * dq/dk/dv are fully overwritten.  */
 int ofk_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
@@ -155,13 +135,12 @@ int ofk_attn_bwd(const void* q, const void* k, const void* v, const void* o, con
                  long long q_bstride, long long ldq, long long k_bstride, long long ldk, long long v_bstride,
                  long long ldv, long long o_bstride, long long ldo, long long dq_bstride, long long lddq,
                  long long dk_bstride, long long lddk, long long dv_bstride, long long lddv, float scale,
-                 int mask_mode, const int* text_time, int keys_per_media, void* workspace, long long workspace_bytes,
-                 void* stream);
+                 int mask_mode, const int* text_time, int keys_per_media, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Dense self-attention core of the frozen LM's decoder blocks (HF MptAttention; reached via
- * flamingo_lm.py:63-65 -- SURVEY.md section 8f rank 1).  head_dim 64 or 128.  Same TMA + tcgen05 implementation
- * (and the same mma.sync path for other layouts) as ofk_attn_fwd / ofk_attn_bwd.
+ * flamingo_lm.py:63-65 -- SURVEY.md section 8f rank 1).  head_dim 64 or 128.  Same wgmma / mma.sync pair as above
+ * (csrc/attention_dense.cu).
  *   S = scale * Q K^T + slopes[h] * key_index  (ALiBi; slopes NULL = no bias)
  *   masked (mask[b, q, k] != 0, mask: [batch, nq, nk] bytes or NULL; and/or causal: key > query + nk - nq)
  *   scores take "finfo.min" exactly like masked_fill: a fully masked row attends uniformly.
@@ -169,7 +148,7 @@ int ofk_attn_bwd(const void* q, const void* k, const void* v, const void* o, con
  *   attention_mask): the kernel then ignores `mask`, applies the causal rule and skips key tiles above the
  *   diagonal -- a device-side decision, so no host synchronisation is needed to pick the fast path.
  *   lse: [batch, heads, nq] f32, log2 domain (consumed only by ofk_attn_dense_bwd).
- * Backward is dgrad only (the LM is frozen): dq/dk/dv bf16, fully overwritten; workspace as for ofk_attn_bwd.
+ * Backward is dgrad only (the LM is frozen): dq/dk/dv bf16, fully overwritten.
  */
 int ofk_attn_dense_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int batch, int heads,
                        int head_dim, int nq, int nk, long long q_bstride, long long ldq, long long k_bstride,
@@ -182,13 +161,12 @@ int ofk_attn_dense_bwd(const void* q, const void* k, const void* v, const void* 
                        long long ldk, long long v_bstride, long long ldv, long long o_bstride, long long ldo,
                        long long dq_bstride, long long lddq, long long dk_bstride, long long lddk,
                        long long dv_bstride, long long lddv, float scale, int causal, const unsigned char* mask,
-                       const float* slopes, const int* pure_causal_flag, void* workspace, long long workspace_bytes,
-                       void* stream);
+                       const float* slopes, const int* pure_causal_flag, void* stream);
 
 /* Attention implementation switch, for A/B measurements and for the parity tests that compare the two paths:
- * nonzero = always use the mma.sync kernels; 0 = tensor-core path whenever the layout allows (the default, unless
- * the environment variable OFK_ATTN_LEGACY=1 is set when the library is loaded).  Returns the previous setting.
- * ofk_attn_tc_launch_count(): how many tcgen05 attention kernels (forward or backward) have been launched. */
+ * nonzero = the mma.sync kernels; 0 = the wgmma kernels (the default, unless the environment variable OFK_ATTN_LEGACY=1
+ * is set when the library is loaded).  Returns the previous setting.
+ * ofk_attn_tc_launch_count(): how many attention calls (forward or backward) the wgmma kernels have served. */
 int ofk_attn_force_legacy(int on);
 long long ofk_attn_tc_launch_count(void);
 
@@ -212,11 +190,17 @@ int ofk_make_labels(const long long* input_ids, long long ld_ids, int batch, int
 /* dst(bf16) = src(f32), n elements (n % 8 == 0 fast path). */
 int ofk_cast_f32_bf16(const float* src, void* dst, long long n, void* stream);
 
+/* Grid-wide sums (dgate, sumsq) write one partial per block into a caller-owned float workspace of at least
+ * ofk_reduce_workspace_bytes() bytes and add the partials in a fixed order, so their results are the same on every
+ * run.  One workspace per stream; it needs no initialisation. */
+long long ofk_reduce_workspace_bytes(void);
+
 /* Gate backward (autograd of helpers.py:274,277):
  *   dbranch(bf16)[i] = dout(f32)[i] * tanh(*gate);  dgate[0] += (1 - tanh(*gate)^2) * sum_i dout[i]*branch(bf16)[i]
- * gate NULL => multiplier 1 and no dgate (plain residual branch, helpers.py:130-131). */
+ * gate NULL => multiplier 1 and no dgate (plain residual branch, helpers.py:130-131).  workspace: see above (may be
+ * NULL when no dgate is wanted). */
 int ofk_gate_bwd(const float* dout, const void* branch, const float* gate, void* dbranch, float* dgate,
-                 long long n, void* stream);
+                 long long n, float* workspace, void* stream);
 
 /* dst(f32) += src(f32) */
 int ofk_add_f32(float* dst, const float* src, long long n, void* stream);
@@ -251,8 +235,8 @@ int ofk_adamw(float* param, const float* grad, float* exp_avg, float* exp_avg_sq
               float lr, float beta1, float beta2, float eps, float wd, float bias_corr1, float bias_corr2,
               const float* clip_scale, const float* step_dev, const float* lr_dev, void* stream);
 
-/* out[0] += sum_i x[i]^2   (global grad norm, train_utils.py:208) */
-int ofk_sumsq(const float* x, long long n, float* out, void* stream);
+/* out[0] += sum_i x[i]^2   (global grad norm, train_utils.py:208); workspace: see ofk_reduce_workspace_bytes. */
+int ofk_sumsq(const float* x, long long n, float* out, float* workspace, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,7 +1,7 @@
-"""In-tree build of libofk.so (sm_100a only) with nvcc.  Used by __graft_entry__.build().
+"""In-tree build of libofk.so (sm_90a only) with nvcc.  Used by __graft_entry__.build().
 
-The library travels to the GPU box with the repo snapshot (it is git-ignored, not gpurun-ignored),
-so nothing is compiled on the GPU box.
+The library is built in the source tree and loaded from there (open_flamingo_b200/libofk.so, git-ignored); nothing is
+compiled at run time.
 """
 import os
 import shutil
@@ -15,7 +15,7 @@ OBJ_DIR = os.path.join(HERE, "csrc", "build")
 LIB_PATH = os.path.join(HERE, "libofk.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -50,7 +50,7 @@ def _stale(target, deps):
 
 
 def build_library(force=False, verbose=False):
-    """Compile every csrc/*.cu for sm_100a and link libofk.so next to this file."""
+    """Compile every csrc/*.cu for sm_90a and link libofk.so next to this file."""
     os.makedirs(OBJ_DIR, exist_ok=True)
     nvcc = _nvcc()
     hdrs = _headers()
@@ -76,7 +76,7 @@ def build_library(force=False, verbose=False):
         with ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(compile_one, jobs))
     if force or jobs or _stale(LIB_PATH, objs):
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_PATH] + objs
+        cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB_PATH] + objs
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -9,10 +9,7 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# OFK_LIB_VARIANT=<name> loads open_flamingo_b200/libofk_<name>.so instead (A/B builds of a kernel made with
-# tools/build_variant.sh; measurement tooling only -- the default and every test use libofk.so)
-_VARIANT = os.environ.get("OFK_LIB_VARIANT", "")
-LIB_PATH = os.path.join(_HERE, f"libofk_{_VARIANT}.so" if _VARIANT else "libofk.so")
+LIB_PATH = os.path.join(_HERE, "libofk.so")
 
 c_void_p = ctypes.c_void_p
 c_int = ctypes.c_int
@@ -43,11 +40,7 @@ _SIGNATURES = {
                               c_int, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_void_p,
                               c_void_p]),
     "ofk_make_labels": (c_int, [c_void_p, c_ll, c_int, c_int, c_ll, c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p]),
-    "ofk_gemm_workspace_bytes": (c_ll, []),
     "ofk_gemm_reserve_sms": (c_int, [c_int]),
-    "ofk_gemm_bf16_ws": (c_int, [c_int, c_int, c_int, c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int,
-                                 c_int, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_void_p,
-                                 c_void_p, c_ll, c_void_p]),
     "ofk_gemm_bf16_grouped": (c_int, [c_int, c_int, c_int, c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int,
                                       c_int, c_void_p, c_ll, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                       c_void_p]),
@@ -60,21 +53,21 @@ _SIGNATURES = {
     "ofk_attn_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                              c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_float, c_int, c_void_p, c_int,
                              c_void_p]),
-    "ofk_attn_bwd_workspace_bytes": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
     "ofk_attn_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                              c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                              c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll,
-                             c_float, c_int, c_void_p, c_int, c_void_p, c_ll, c_void_p]),
+                             c_float, c_int, c_void_p, c_int, c_void_p]),
     "ofk_attn_dense_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                    c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_ll, c_float, c_int, c_void_p, c_void_p,
                                    c_void_p, c_void_p]),
     "ofk_attn_dense_bwd": (c_int, [c_void_p] * 10 + [c_int] * 5 + [c_ll] * 14 + [c_float, c_int, c_void_p, c_void_p,
-                                                                              c_void_p, c_void_p, c_ll, c_void_p]),
+                                                                              c_void_p, c_void_p]),
     "ofk_attn_force_legacy": (c_int, [c_int]),
     "ofk_attn_tc_launch_count": (c_ll, []),
     "ofk_text_time": (c_int, [c_void_p, c_ll, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "ofk_cast_f32_bf16": (c_int, [c_void_p, c_void_p, c_ll, c_void_p]),
-    "ofk_gate_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p]),
+    "ofk_reduce_workspace_bytes": (c_ll, []),
+    "ofk_gate_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_void_p]),
     "ofk_add_f32": (c_int, [c_void_p, c_void_p, c_ll, c_void_p]),
     "ofk_patchify": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_ll, c_void_p]),
     "ofk_vit_assemble": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
@@ -84,7 +77,7 @@ _SIGNATURES = {
                            c_void_p, c_ll, c_void_p]),
     "ofk_adamw": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_float, c_float, c_float,
                           c_float, c_float, c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "ofk_sumsq": (c_int, [c_void_p, c_ll, c_void_p, c_void_p]),
+    "ofk_sumsq": (c_int, [c_void_p, c_ll, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None
@@ -102,13 +95,13 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a).  There is no CPU/PyTorch fallback for the hot path.")
+                "(nvcc, sm_90a).  There is no CPU/PyTorch fallback for the hot path.")
         L = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in _SIGNATURES.items():
             fn = getattr(L, name)  # AttributeError if the symbol is not exported
             fn.restype = res
             fn.argtypes = args
-        if L.ofk_abi_version() != 2:
+        if L.ofk_abi_version() != 3:
             raise RuntimeError("libofk.so ABI version mismatch")
         _lib = L
     return _lib
@@ -140,7 +133,7 @@ def require_cuda(*tensors):
         if t is None:
             continue
         if not t.is_cuda:
-            raise RuntimeError("open_flamingo_b200 kernels need CUDA tensors (sm_100a); there is no CPU path")
+            raise RuntimeError("open_flamingo_b200 kernels need CUDA tensors (sm_90a); there is no CPU path")
         if cur is None:
             cur = torch.cuda.current_device()
         if t.device.index != cur:

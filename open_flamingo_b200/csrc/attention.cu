@@ -19,7 +19,6 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "attention_tc.h"
 #include "ofk_internal.h"
 #include "ofk_ptx.cuh"
 
@@ -45,6 +44,7 @@ struct AttnParams {
 };
 
 // ---------------------------------------------------------------- smem tile helpers (64 rows x 64 bf16, swizzled)
+// The XOR pattern is the 128-byte swizzle wgmma descriptors expect; tiles start on 1024-byte boundaries.
 __device__ __forceinline__ uint32_t tile_off(int row, int chunk) {  // chunk = 16-byte column group 0..7
   return (uint32_t)(row * 128 + ((chunk ^ (row & 7)) << 4));
 }
@@ -97,38 +97,75 @@ __device__ __forceinline__ void load_a_frags(const uint8_t* tile, int r0, uint32
   }
 }
 
-// C[16 x 64] (+)= A[16 x 64(k)] * T^T where T is a [64 n][64 k] row-major tile  ("n rows, k contiguous").
-__device__ __forceinline__ void mma_a_tileT(float (&c)[8][4], const uint32_t (&a)[4][4], const uint8_t* tile) {
-  const int lane = threadIdx.x & 31;
+// Tensor-core products of one CTA = one warpgroup of 4 warps x 16 rows.  WG = true: one warpgroup-wide wgmma per 16-deep
+// k step over all 64 rows (A from each warp's registers, B from the 128-byte-swizzled tile through a descriptor);
+// WG = false: per-warp mma.sync, kept as the A/B reference.  Both use the same accumulator and A-fragment layout, so
+// the softmax / mask code around them is shared.
+__device__ __forceinline__ void wgmma_pin(float* d, int n) {
+  for (int i = 0; i < n; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// C[16 x 64] (+)= A[16 x 64(k)] * T^T where T is a [64 n][64 k] row-major tile  ("n rows, k contiguous").  A is the
+// warp's rows of `atile` (WG: read by wgmma through a descriptor of the whole 64-row tile) or, for mma.sync, the
+// fragments `a` already loaded from it.
+template <bool WG>
+__device__ __forceinline__ void mma_a_tileT(float (&c)[8][4], const uint32_t (&a)[4][4], const uint8_t* atile,
+                                            const uint8_t* tile) {
   const uint32_t base = smem_u32(tile);
+  if constexpr (WG) {
+    const uint32_t abase = smem_u32(atile);
+    float(&d)[32] = *reinterpret_cast<float(*)[32]>(&c[0][0]);
+    wgmma_pin(d, 32);
+    wgmma_fence();
 #pragma unroll
-  for (int np = 0; np < 4; ++np) {       // pairs of 8-wide n tiles
-    const int nrow = np * 16 + (lane & 7) + (lane >> 4) * 8;
+    for (int ks = 0; ks < 4; ++ks)
+      wgmma_m64n64k16_ss(d, make_wgmma_desc_sw128(abase + ks * 32, 16, 1024), make_wgmma_desc_sw128(base + ks * 32, 16, 1024));
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_pin(d, 32);
+  } else {
+    const int lane = threadIdx.x & 31;
 #pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      uint32_t b0, b1, b2, b3;
-      const int chunk = ks * 2 + ((lane >> 3) & 1);
-      ldsm_x4(base + tile_off(nrow, chunk), b0, b1, b2, b3);
-      mma16816(c[np * 2], a[ks], b0, b1);
-      mma16816(c[np * 2 + 1], a[ks], b2, b3);
+    for (int np = 0; np < 4; ++np) {       // pairs of 8-wide n tiles
+      const int nrow = np * 16 + (lane & 7) + (lane >> 4) * 8;
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        uint32_t b0, b1, b2, b3;
+        const int chunk = ks * 2 + ((lane >> 3) & 1);
+        ldsm_x4(base + tile_off(nrow, chunk), b0, b1, b2, b3);
+        mma16816(c[np * 2], a[ks], b0, b1);
+        mma16816(c[np * 2 + 1], a[ks], b2, b3);
+      }
     }
   }
 }
 
 // C[16 x 64(n)] += P[16 x 64(k)] * T where T is a [64 k][64 n] row-major tile ("k rows, n contiguous").
+template <bool WG>
 __device__ __forceinline__ void mma_p_tile(float (&c)[8][4], const uint32_t (&p)[4][4], const uint8_t* tile) {
-  const int lane = threadIdx.x & 31;
   const uint32_t base = smem_u32(tile);
+  if constexpr (WG) {
+    float(&d)[32] = *reinterpret_cast<float(*)[32]>(&c[0][0]);
+    wgmma_pin(d, 32);
+    wgmma_fence();
 #pragma unroll
-  for (int ks = 0; ks < 4; ++ks) {
-    const int krow = ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+    for (int ks = 0; ks < 4; ++ks) wgmma_m64n64k16_rs<1>(d, p[ks], make_wgmma_desc_sw128(base + ks * 2048, 8192, 1024));
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_pin(d, 32);
+  } else {
+    const int lane = threadIdx.x & 31;
 #pragma unroll
-    for (int np = 0; np < 4; ++np) {
-      uint32_t b0, b1, b2, b3;
-      const int chunk = np * 2 + (lane >> 4);
-      ldsm_x4_t(base + tile_off(krow, chunk), b0, b1, b2, b3);
-      mma16816(c[np * 2], p[ks], b0, b1);
-      mma16816(c[np * 2 + 1], p[ks], b2, b3);
+    for (int ks = 0; ks < 4; ++ks) {
+      const int krow = ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+#pragma unroll
+      for (int np = 0; np < 4; ++np) {
+        uint32_t b0, b1, b2, b3;
+        const int chunk = np * 2 + (lane >> 4);
+        ldsm_x4_t(base + tile_off(krow, chunk), b0, b1, b2, b3);
+        mma16816(c[np * 2], p[ks], b0, b1);
+        mma16816(c[np * 2 + 1], p[ks], b2, b3);
+      }
     }
   }
 }
@@ -206,10 +243,16 @@ __device__ __forceinline__ void block_key_range(const AttnParams& p, int b, int 
 }
 
 // ================================================================ forward
+// Tiles live in dynamic shared memory aligned by hand: the 128-byte swizzle wgmma reads is a function of the absolute
+// shared address, so every tile must start on a 1024-byte boundary.
+constexpr int FWD_SMEM = 5 * 64 * 128 + 1024;
+extern __shared__ uint8_t att_dyn_smem[];
+template <bool WG>
 __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnParams p) {
-  __shared__ __align__(128) uint8_t sQ[BQ * 128];
-  __shared__ __align__(128) uint8_t sK[2][BKV * 128];
-  __shared__ __align__(128) uint8_t sV[2][BKV * 128];
+  uint8_t* fbase = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(att_dyn_smem) + 1023) & ~uintptr_t(1023));
+  uint8_t* sQ = fbase;
+  uint8_t* sK[2] = {fbase + 64 * 128, fbase + 2 * 64 * 128};
+  uint8_t* sV[2] = {fbase + 3 * 64 * 128, fbase + 4 * 64 * 128};
   __shared__ int s_red[12];
 
   const int q0 = blockIdx.x * BQ, h = blockIdx.y, b = blockIdx.z;
@@ -246,13 +289,14 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnParams 
     } else {
       cp_async_wait<0>();
     }
+    if constexpr (WG) fence_proxy_async_smem();   // cp.async (generic proxy) -> wgmma reads
     __syncthreads();
-    if (j == 0) load_a_frags(sQ, warp * 16, qa);
+    if (!WG && j == 0) load_a_frags(sQ, warp * 16, qa);
 
     float s[8][4];
 #pragma unroll
     for (int i = 0; i < 8; ++i) { s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f; }
-    mma_a_tileT(s, qa, sK[buf]);
+    mma_a_tileT<WG>(s, qa, sQ, sK[buf]);
 
     // mask + scale (log2 domain)
     const int key0 = klo + j * BKV;
@@ -304,7 +348,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnParams 
     for (int i = 0; i < 8; ++i) { o[i][0] *= corr_a; o[i][1] *= corr_a; o[i][2] *= corr_b; o[i][3] *= corr_b; }
     uint32_t pa[4][4];
     c_to_a(s, pa);
-    mma_p_tile(o, pa, sV[buf]);
+    mma_p_tile<WG>(o, pa, sV[buf]);
     __syncthreads();
   }
   if (nblk == 0) { cp_async_wait<0>(); }
@@ -320,8 +364,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnParams 
     if (row_b < p.nq) *reinterpret_cast<uint32_t*>(op + (long long)row_b * p.ldo + col) = pack_bf16x2(o[i][2] * inv_b, o[i][3] * inv_b);
   }
   if (p.lse != nullptr && t == 0) {
-    // log2-domain LSE of the scaled scores (same convention as the tcgen05 kernels of attention_tc.cu, so either
-    // backward can consume either forward); rows with no mass get the sentinel 0 (P recomputes to 0 there because
+    // log2-domain LSE of the scaled scores; rows with no mass get the sentinel 0 (P recomputes to 0 there because
     // every score is -inf).
     float* lp = p.lse + ((long long)b * p.heads + h) * p.nq;
     if (row_a < p.nq) lp[row_a] = l_a > 0.f ? m_a + log2f(l_a) : 0.f;
@@ -382,11 +425,11 @@ __device__ __forceinline__ void recompute_p(const AttnParams& p, float (&s)[8][4
 }
 
 // ================================================================ backward: dQ  (CTA = 64 queries, loop over key tiles)
-constexpr int BWD_SMEM = 6 * 64 * 128 + 128;  // six 8 KiB tiles + alignment slack
-extern __shared__ uint8_t att_dyn_smem[];
+constexpr int BWD_SMEM = 6 * 64 * 128 + 1024;  // six 8 KiB tiles + alignment slack
 
+template <bool WG>
 __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnParams p) {
-  uint8_t* base_ = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(att_dyn_smem) + 127) & ~uintptr_t(127));
+  uint8_t* base_ = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(att_dyn_smem) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = base_;
   uint8_t* sdO = base_ + 8192;
   uint8_t* sK[2] = {base_ + 2 * 8192, base_ + 3 * 8192};
@@ -431,14 +474,15 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
     } else {
       cp_async_wait<0>();
     }
+    if constexpr (WG) fence_proxy_async_smem();   // cp.async (generic proxy) -> wgmma reads
     __syncthreads();
-    if (j == 0) { load_a_frags(sQ, warp * 16, qa); load_a_frags(sdO, warp * 16, doa); }
+    if (!WG && j == 0) { load_a_frags(sQ, warp * 16, qa); load_a_frags(sdO, warp * 16, doa); }
 
     float s[8][4], dpv[8][4];
 #pragma unroll
     for (int i = 0; i < 8; ++i) { s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f; dpv[i][0] = dpv[i][1] = dpv[i][2] = dpv[i][3] = 0.f; }
-    mma_a_tileT(s, qa, sK[buf]);      // S  = Q K^T
-    mma_a_tileT(dpv, doa, sV[buf]);   // dP = dO V^T
+    mma_a_tileT<WG>(s, qa, sQ, sK[buf]);      // S  = Q K^T
+    mma_a_tileT<WG>(dpv, doa, sdO, sV[buf]);   // dP = dO V^T
     recompute_p(p, s, ra, rb, lse_a, lse_b, klo + j * BKV, t);
     const float ga = ra.kind == 2 ? 0.f : p.scale, gb = rb.kind == 2 ? 0.f : p.scale;
 #pragma unroll
@@ -448,7 +492,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
     }
     uint32_t dsa[4][4];
     c_to_a(s, dsa);
-    mma_p_tile(dq, dsa, sK[buf]);     // dQ += dS K
+    mma_p_tile<WG>(dq, dsa, sK[buf]);     // dQ += dS K
     __syncthreads();
   }
   if (nblk == 0) { cp_async_wait<0>(); }
@@ -465,8 +509,9 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
 // ================================================================ backward: dK, dV (CTA = 64 keys, loop over query tiles)
 // Works on transposed tiles: S^T = K Q^T (rows = keys), so P^T / dS^T are directly the A operands of
 // dV += P^T dO and dK += dS^T Q.
+template <bool WG>
 __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const AttnParams p) {
-  uint8_t* base_ = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(att_dyn_smem) + 127) & ~uintptr_t(127));
+  uint8_t* base_ = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(att_dyn_smem) + 1023) & ~uintptr_t(1023));
   uint8_t* sK = base_;
   uint8_t* sV = base_ + 8192;
   uint8_t* sQ[2] = {base_ + 2 * 8192, base_ + 3 * 8192};
@@ -520,6 +565,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const AttnPar
     } else {
       cp_async_wait<0>();
     }
+    if constexpr (WG) fence_proxy_async_smem();   // cp.async (generic proxy) -> wgmma reads
     __syncthreads();
     {
       // skip (query block, key block) pairs the media mask rules out entirely
@@ -540,10 +586,10 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const AttnPar
     for (int i = 0; i < 8; ++i) { st[i][0] = st[i][1] = st[i][2] = st[i][3] = 0.f; dpt[i][0] = dpt[i][1] = dpt[i][2] = dpt[i][3] = 0.f; }
     {
       uint32_t fa[4][4];              // A fragments are re-read from smem each time: keeps the kernel under 255 regs
-      load_a_frags(sK, warp * 16, fa);
-      mma_a_tileT(st, fa, sQ[buf]);     // S^T  = K Q^T   [16 keys x 64 queries]
-      load_a_frags(sV, warp * 16, fa);
-      mma_a_tileT(dpt, fa, sdO[buf]);   // dP^T = V dO^T
+      if (!WG) load_a_frags(sK, warp * 16, fa);
+      mma_a_tileT<WG>(st, fa, sK, sQ[buf]);     // S^T  = K Q^T   [16 keys x 64 queries]
+      if (!WG) load_a_frags(sV, warp * 16, fa);
+      mma_a_tileT<WG>(dpt, fa, sV, sdO[buf]);   // dP^T = V dO^T
     }
     float dst[8][4];
 #pragma unroll
@@ -562,8 +608,8 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const AttnPar
     uint32_t pa[4][4], dsa[4][4];
     c_to_a(st, pa);
     c_to_a(dst, dsa);
-    mma_p_tile(dv, pa, sdO[buf]);     // dV += P^T dO
-    mma_p_tile(dk, dsa, sQ[buf]);     // dK += dS^T Q
+    mma_p_tile<WG>(dv, pa, sdO[buf]);     // dV += P^T dO
+    mma_p_tile<WG>(dk, dsa, sQ[buf]);     // dK += dS^T Q
     __syncthreads();
   }
 
@@ -611,34 +657,15 @@ extern "C" int ofk_attn_fwd(const void* q, const void* k, const void* v, void* o
   p.o_bs = o_bstride; p.ldo = ldo; p.scale = scale; p.mask_mode = mask_mode; p.kpm = keys_per_media;
   if (!q || !k || !v || !o) return ofk_set_error(OFK_ERR_ARG, "attention: null pointer");
   if (int rc = check_common(p)) return rc;
-  {
-    // default path: TMA + tcgen05 (attention_tc.cu); the mma.sync kernel below serves layouts TMA cannot describe
-    tc::Args a{};
-    a.q = q; a.k = k; a.v = v; a.out = o; a.lse = lse; a.batch = batch; a.heads = heads; a.hd = HD; a.nq = nq; a.nk = nk;
-    a.q_bs = q_bstride; a.ldq = ldq; a.k_bs = k_bstride; a.ldk = ldk; a.v_bs = v_bstride; a.ldv = ldv; a.o_bs = o_bstride;
-    a.ldo = ldo; a.scale = scale; a.dense = 0; a.mask_mode = mask_mode; a.text_time = text_time; a.kpm = keys_per_media;
-    a.stream = stream_;
-    if (tc::fwd_supported(a)) {
-      // A sequence that overhangs the last 128-query tile by a few rows (the ViT's 257 = 2 x 128 + 1 tokens) would cost
-      // a whole extra tile -- a third of the CTAs -- for those rows: the tensor-core kernel takes the full tiles and
-      // the overhanging rows go through the 64-row mma.sync kernel below (no mask, no LSE: the ViT forward).
-      const int tail = nq % 128;
-      if (nq > 128 && tail > 0 && tail <= 16 && mask_mode == 0 && lse == nullptr) {
-        a.q_tile_limit = nq / 128;
-        if (int rc = tc::fwd(a)) return rc;
-        const long long r0 = (long long)(nq - tail);
-        p.q += r0 * ldq; p.out += r0 * ldo; p.nq = tail;
-        dim3 grid_t(1, heads, batch);
-        attn_fwd_kernel<<<grid_t, ATT_THREADS, 0, (cudaStream_t)stream_>>>(p);
-        OFK_CHECK_LAUNCH();
-        return 0;
-      }
-      return tc::fwd(a);
-    }
-  }
   dim3 grid((nq + BQ - 1) / BQ, heads, batch);
-  attn_fwd_kernel<<<grid, ATT_THREADS, 0, (cudaStream_t)stream_>>>(p);
-  OFK_CHECK_LAUNCH();
+  if (ofk_attn_use_wgmma()) {
+    attn_fwd_kernel<true><<<grid, ATT_THREADS, FWD_SMEM, (cudaStream_t)stream_>>>(p);
+    OFK_CHECK_LAUNCH();
+    ofk_attn_count_wgmma();
+  } else {
+    attn_fwd_kernel<false><<<grid, ATT_THREADS, FWD_SMEM, (cudaStream_t)stream_>>>(p);
+    OFK_CHECK_LAUNCH();
+  }
   return 0;
 }
 
@@ -648,7 +675,7 @@ extern "C" int ofk_attn_bwd(const void* q, const void* k, const void* v, const v
                             long long v_bstride, long long ldv, long long o_bstride, long long ldo,
                             long long dq_bstride, long long lddq, long long dk_bstride, long long lddk,
                             long long dv_bstride, long long lddv, float scale, int mask_mode, const int* text_time,
-                            int keys_per_media, void* workspace, long long workspace_bytes, void* stream_) {
+                            int keys_per_media, void* stream_) {
   using namespace ofk;
   AttnParams p{};
   p.q = (const __nv_bfloat16*)q; p.k = (const __nv_bfloat16*)k; p.v = (const __nv_bfloat16*)v;
@@ -662,16 +689,6 @@ extern "C" int ofk_attn_bwd(const void* q, const void* k, const void* v, const v
     return ofk_set_error(OFK_ERR_ARG, "attention bwd: null pointer");
   if (int rc = check_common(p)) return rc;
   if ((lddq | lddk | lddv) % 2 != 0) return ofk_set_error(OFK_ERR_ALIGN, "attention bwd: grad strides must be even");
-  {
-    tc::Args a{};
-    a.q = q; a.k = k; a.v = v; a.o = o; a.d_o = d_o; a.lse = const_cast<float*>(lse); a.delta = delta; a.dq = dq; a.dk = dk;
-    a.dv = dv; a.batch = batch; a.heads = heads; a.hd = HD; a.nq = nq; a.nk = nk;
-    a.q_bs = q_bstride; a.ldq = ldq; a.k_bs = k_bstride; a.ldk = ldk; a.v_bs = v_bstride; a.ldv = ldv; a.o_bs = o_bstride;
-    a.ldo = ldo; a.dq_bs = dq_bstride; a.lddq = lddq; a.dk_bs = dk_bstride; a.lddk = lddk; a.dv_bs = dv_bstride; a.lddv = lddv;
-    a.scale = scale; a.dense = 0; a.mask_mode = mask_mode; a.text_time = text_time; a.kpm = keys_per_media;
-    a.workspace = workspace; a.workspace_bytes = workspace_bytes; a.stream = stream_;
-    if (tc::bwd_supported(a)) return tc::bwd(a);
-  }
   cudaStream_t stream = (cudaStream_t)stream_;
   const long long rows = (long long)batch * heads * nq;
   attn_delta_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(p);
@@ -679,14 +696,24 @@ extern "C" int ofk_attn_bwd(const void* q, const void* k, const void* v, const v
   dim3 gq((nq + BQ - 1) / BQ, heads, batch);
   static bool attr_done = false;
   if (!attr_done) {
-    cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
-    cudaFuncSetAttribute(attn_bwd_dkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
+    cudaFuncSetAttribute(attn_bwd_dq_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
+    cudaFuncSetAttribute(attn_bwd_dkv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
+    cudaFuncSetAttribute(attn_bwd_dq_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
+    cudaFuncSetAttribute(attn_bwd_dkv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
     attr_done = true;
   }
-  attn_bwd_dq_kernel<<<gq, ATT_THREADS, BWD_SMEM, stream>>>(p);
-  OFK_CHECK_LAUNCH();
   dim3 gk((nk + BKV - 1) / BKV, heads, batch);
-  attn_bwd_dkv_kernel<<<gk, ATT_THREADS, BWD_SMEM, stream>>>(p);
-  OFK_CHECK_LAUNCH();
+  if (ofk_attn_use_wgmma()) {
+    attn_bwd_dq_kernel<true><<<gq, ATT_THREADS, BWD_SMEM, stream>>>(p);
+    OFK_CHECK_LAUNCH();
+    attn_bwd_dkv_kernel<true><<<gk, ATT_THREADS, BWD_SMEM, stream>>>(p);
+    OFK_CHECK_LAUNCH();
+    ofk_attn_count_wgmma();
+  } else {
+    attn_bwd_dq_kernel<false><<<gq, ATT_THREADS, BWD_SMEM, stream>>>(p);
+    OFK_CHECK_LAUNCH();
+    attn_bwd_dkv_kernel<false><<<gk, ATT_THREADS, BWD_SMEM, stream>>>(p);
+    OFK_CHECK_LAUNCH();
+  }
   return 0;
 }

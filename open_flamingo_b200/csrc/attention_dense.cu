@@ -14,7 +14,6 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "attention_tc.h"
 #include "ofk_internal.h"
 #include "ofk_ptx.cuh"
 
@@ -46,8 +45,10 @@ struct Tile {
   static constexpr int BYTES = 64 * ROW_BYTES;  // 64-row tile
   static constexpr int KSTEPS = HD / 16;       // k-steps when HD is the contraction dim
   static constexpr int NT = HD / 8;            // 8-wide n tiles when HD is the output dim
+  // 64-column halves of the tile are separate 8 KiB atoms of 64 rows x 128 bytes with the 128-byte XOR swizzle: the
+  // canonical layout wgmma descriptors read (tiles start on 1024-byte boundaries).
   __device__ static __forceinline__ uint32_t off(int row, int chunk) {
-    return (uint32_t)(row * ROW_BYTES + ((chunk ^ (row & 7)) << 4));
+    return (uint32_t)((chunk >> 3) * (64 * 128) + row * 128 + (((chunk & 7) ^ (row & 7)) << 4));
   }
 };
 
@@ -83,44 +84,80 @@ __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], 
                : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// C[16 x 64] += X[rows r0.., HD(k)] * T^T, both [rows][HD] tiles (contraction over HD).  A fragments are loaded
-// from `xt` on the fly (keeps registers free).
-template <int HD>
+__device__ __forceinline__ void wgmma_pin(float* d, int n) {
+  for (int i = 0; i < n; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// Tensor-core products of one CTA = one warpgroup of 4 warps x 16 rows.  WG = true: warpgroup-wide wgmma over all 64
+// rows, operands from the swizzled tiles through descriptors (P / dS from registers); WG = false: per-warp mma.sync,
+// kept as the A/B reference.  Both share the accumulator and A-fragment layout, so the code around them is common.
+
+// C[16 x 64] += X[rows r0.., HD(k)] * T^T, both [rows][HD] tiles (contraction over HD).
+template <int HD, bool WG>
 __device__ __forceinline__ void mma_rows_x_tileT(float (&c)[8][4], const uint8_t* xt, int r0, const uint8_t* tile) {
   using T = Tile<HD>;
-  const int lane = threadIdx.x & 31;
   const uint32_t xb = smem_u32(xt), tb = smem_u32(tile);
-  const int arow = r0 + (lane & 7) + ((lane >> 3) & 1) * 8;
+  if constexpr (WG) {
+    float(&d)[32] = *reinterpret_cast<float(*)[32]>(&c[0][0]);
+    wgmma_pin(d, 32);
+    wgmma_fence();
 #pragma unroll
-  for (int ks = 0; ks < T::KSTEPS; ++ks) {
-    uint32_t a[4];
-    ldsm4(xb + T::off(arow, ks * 2 + (lane >> 4)), a[0], a[1], a[2], a[3]);
+    for (int ks = 0; ks < T::KSTEPS; ++ks) {
+      const uint32_t o = (ks >> 2) * (64 * 128) + (ks & 3) * 32;
+      wgmma_m64n64k16_ss(d, make_wgmma_desc_sw128(xb + o, 16, 1024), make_wgmma_desc_sw128(tb + o, 16, 1024));
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_pin(d, 32);
+  } else {
+    const int lane = threadIdx.x & 31;
+    const int arow = r0 + (lane & 7) + ((lane >> 3) & 1) * 8;
 #pragma unroll
-    for (int np = 0; np < 4; ++np) {
-      const int nrow = np * 16 + (lane & 7) + (lane >> 4) * 8;
-      uint32_t b0, b1, b2, b3;
-      ldsm4(tb + T::off(nrow, ks * 2 + ((lane >> 3) & 1)), b0, b1, b2, b3);
-      mma16816(c[np * 2], a, b0, b1);
-      mma16816(c[np * 2 + 1], a, b2, b3);
+    for (int ks = 0; ks < T::KSTEPS; ++ks) {
+      uint32_t a[4];
+      ldsm4(xb + T::off(arow, ks * 2 + (lane >> 4)), a[0], a[1], a[2], a[3]);
+#pragma unroll
+      for (int np = 0; np < 4; ++np) {
+        const int nrow = np * 16 + (lane & 7) + (lane >> 4) * 8;
+        uint32_t b0, b1, b2, b3;
+        ldsm4(tb + T::off(nrow, ks * 2 + ((lane >> 3) & 1)), b0, b1, b2, b3);
+        mma16816(c[np * 2], a, b0, b1);
+        mma16816(c[np * 2 + 1], a, b2, b3);
+      }
     }
   }
 }
 
 // C[16 x HD] += P[16 x 64(k)] * T, T = [64 k][HD n] tile (contraction over the tile's 64 rows).
-template <int HD>
+template <int HD, bool WG>
 __device__ __forceinline__ void mma_p_x_tile(float (&c)[Tile<HD>::NT][4], const uint32_t (&p)[4][4], const uint8_t* tile) {
   using T = Tile<HD>;
-  const int lane = threadIdx.x & 31;
   const uint32_t tb = smem_u32(tile);
+  if constexpr (WG) {
+    float(&d)[T::NT * 4] = *reinterpret_cast<float(*)[T::NT * 4]>(&c[0][0]);
+    wgmma_pin(d, T::NT * 4);
+    wgmma_fence();
 #pragma unroll
-  for (int ks = 0; ks < 4; ++ks) {
-    const int krow = ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+    for (int ks = 0; ks < 4; ++ks) {
+      const uint64_t bd = make_wgmma_desc_sw128(tb + ks * 2048, 64 * 128, 1024);   // MN-major: atoms 8 KiB apart
+      if constexpr (HD == 64) wgmma_m64n64k16_rs<1>(d, p[ks], bd);
+      else wgmma_m64n128k16_rs<1>(d, p[ks], bd);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_pin(d, T::NT * 4);
+  } else {
+    const int lane = threadIdx.x & 31;
 #pragma unroll
-    for (int np = 0; np < T::NT / 2; ++np) {
-      uint32_t b0, b1, b2, b3;
-      ldsm4t(tb + T::off(krow, np * 2 + (lane >> 4)), b0, b1, b2, b3);
-      mma16816(c[np * 2], p[ks], b0, b1);
-      mma16816(c[np * 2 + 1], p[ks], b2, b3);
+    for (int ks = 0; ks < 4; ++ks) {
+      const int krow = ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+#pragma unroll
+      for (int np = 0; np < T::NT / 2; ++np) {
+        uint32_t b0, b1, b2, b3;
+        ldsm4t(tb + T::off(krow, np * 2 + (lane >> 4)), b0, b1, b2, b3);
+        mma16816(c[np * 2], p[ks], b0, b1);
+        mma16816(c[np * 2 + 1], p[ks], b2, b3);
+      }
     }
   }
 }
@@ -133,6 +170,18 @@ __device__ __forceinline__ void c_to_a(const float (&c)[8][4], uint32_t (&a)[4][
     a[ks][2] = pack_bf16x2(c[2 * ks + 1][0], c[2 * ks + 1][1]);
     a[ks][3] = pack_bf16x2(c[2 * ks + 1][2], c[2 * ks + 1][3]);
   }
+}
+
+// P as hi + lo bf16 fragments (lo = P - bf16(P), exact in fp32): O += P_hi V + P_lo V carries P to ~16 mantissa bits
+// instead of 8.  A single bf16 rounding of P here, compounded over the LM's decoder blocks, was measured to bias the
+// gradient reaching the first gated block by 1-2 % against fp32 (the gate-gradient parity test).
+__device__ __forceinline__ void c_to_a_split(float (&c)[8][4], uint32_t (&hi)[4][4], uint32_t (&lo)[4][4]) {
+  c_to_a(c, hi);
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) c[i][e] -= bf16_round(c[i][e]);
+  c_to_a(c, lo);
 }
 
 // log2-domain score of (row, key) given the raw dot product.
@@ -165,12 +214,12 @@ __device__ __forceinline__ bool tile_unmasked(const Params& p, int key_last, int
 extern __shared__ uint8_t dyn_smem[];
 
 // ================================================================ forward
-template <int HD>
+template <int HD, bool WG>
 __global__ void __launch_bounds__(THREADS) fwd_kernel(const Params p_in) {
   Params p = p_in;
   if (p.pure_causal != nullptr && *p.pure_causal != 0) { p.mask = nullptr; p.causal = 1; }
   using T = Tile<HD>;
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(dyn_smem) + 127) & ~uintptr_t(127));
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(dyn_smem) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = base;
   uint8_t* sK[2] = {base + T::BYTES, base + 2 * T::BYTES};
   uint8_t* sV[2] = {base + 3 * T::BYTES, base + 4 * T::BYTES};
@@ -204,11 +253,12 @@ __global__ void __launch_bounds__(THREADS) fwd_kernel(const Params p_in) {
     } else {
       cp_wait<0>();
     }
+    if constexpr (WG) fence_proxy_async_smem();   // cp.async (generic proxy) -> wgmma reads
     __syncthreads();
     float s[8][4];
 #pragma unroll
     for (int i = 0; i < 8; ++i) { s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f; }
-    mma_rows_x_tileT<HD>(s, sQ, warp * 16, sK[buf]);
+    mma_rows_x_tileT<HD, WG>(s, sQ, warp * 16, sK[buf]);
     float mx_a = -INFINITY, mx_b = -INFINITY;
     if (tile_unmasked(p, j * BKV + BKV - 1, q0 + warp * 16)) {
       const float kb = slope2 * (float)(j * BKV + 2 * t);
@@ -248,9 +298,10 @@ __global__ void __launch_bounds__(THREADS) fwd_kernel(const Params p_in) {
     l_a = l_a * corr_a + rs_a; l_b = l_b * corr_b + rs_b;
 #pragma unroll
     for (int i = 0; i < T::NT; ++i) { o[i][0] *= corr_a; o[i][1] *= corr_a; o[i][2] *= corr_b; o[i][3] *= corr_b; }
-    uint32_t pa[4][4];
-    c_to_a(s, pa);
-    mma_p_x_tile<HD>(o, pa, sV[buf]);
+    uint32_t pa[4][4], pl[4][4];
+    c_to_a_split(s, pa, pl);
+    mma_p_x_tile<HD, WG>(o, pa, sV[buf]);
+    mma_p_x_tile<HD, WG>(o, pl, sV[buf]);
     __syncthreads();
   }
   if (nblk == 0) cp_wait<0>();
@@ -294,12 +345,12 @@ __global__ void delta_kernel(const Params p) {
 }
 
 // ================================================================ dQ (CTA = 64 queries, loop key tiles)
-template <int HD>
+template <int HD, bool WG>
 __global__ void __launch_bounds__(THREADS) bwd_dq_kernel(const Params p_in) {
   Params p = p_in;
   if (p.pure_causal != nullptr && *p.pure_causal != 0) { p.mask = nullptr; p.causal = 1; }
   using T = Tile<HD>;
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(dyn_smem) + 127) & ~uintptr_t(127));
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(dyn_smem) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = base;
   uint8_t* sdO = base + T::BYTES;
   uint8_t* sK[2] = {base + 2 * T::BYTES, base + 3 * T::BYTES};
@@ -339,12 +390,13 @@ __global__ void __launch_bounds__(THREADS) bwd_dq_kernel(const Params p_in) {
     } else {
       cp_wait<0>();
     }
+    if constexpr (WG) fence_proxy_async_smem();   // cp.async (generic proxy) -> wgmma reads
     __syncthreads();
     float s[8][4], dpv[8][4];
 #pragma unroll
     for (int i = 0; i < 8; ++i) { s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f; dpv[i][0] = dpv[i][1] = dpv[i][2] = dpv[i][3] = 0.f; }
-    mma_rows_x_tileT<HD>(s, sQ, warp * 16, sK[buf]);     // S  = Q K^T
-    mma_rows_x_tileT<HD>(dpv, sdO, warp * 16, sV[buf]);  // dP = dO V^T
+    mma_rows_x_tileT<HD, WG>(s, sQ, warp * 16, sK[buf]);     // S  = Q K^T
+    mma_rows_x_tileT<HD, WG>(dpv, sdO, warp * 16, sV[buf]);  // dP = dO V^T
     if (tile_unmasked(p, j * BKV + BKV - 1, q0 + warp * 16)) {
       const float kb = slope2 * (float)(j * BKV + 2 * t);
 #pragma unroll
@@ -371,7 +423,7 @@ __global__ void __launch_bounds__(THREADS) bwd_dq_kernel(const Params p_in) {
     }
     uint32_t dsa[4][4];
     c_to_a(s, dsa);
-    mma_p_x_tile<HD>(dq, dsa, sK[buf]);                  // dQ += dS K
+    mma_p_x_tile<HD, WG>(dq, dsa, sK[buf]);                  // dQ += dS K
     __syncthreads();
   }
   if (nblk == 0) cp_wait<0>();
@@ -386,12 +438,12 @@ __global__ void __launch_bounds__(THREADS) bwd_dq_kernel(const Params p_in) {
 }
 
 // ================================================================ dK, dV (CTA = 64 keys, loop query tiles)
-template <int HD>
+template <int HD, bool WG>
 __global__ void __launch_bounds__(THREADS) bwd_dkv_kernel(const Params p_in) {
   Params p = p_in;
   if (p.pure_causal != nullptr && *p.pure_causal != 0) { p.mask = nullptr; p.causal = 1; }
   using T = Tile<HD>;
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(dyn_smem) + 127) & ~uintptr_t(127));
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(dyn_smem) + 1023) & ~uintptr_t(1023));
   uint8_t* sK = base;
   uint8_t* sV = base + T::BYTES;
   uint8_t* sQ[2] = {base + 2 * T::BYTES, base + 3 * T::BYTES};
@@ -443,12 +495,13 @@ __global__ void __launch_bounds__(THREADS) bwd_dkv_kernel(const Params p_in) {
     } else {
       cp_wait<0>();
     }
+    if constexpr (WG) fence_proxy_async_smem();   // cp.async (generic proxy) -> wgmma reads
     __syncthreads();
     float st[8][4], dpt[8][4];
 #pragma unroll
     for (int i = 0; i < 8; ++i) { st[i][0] = st[i][1] = st[i][2] = st[i][3] = 0.f; dpt[i][0] = dpt[i][1] = dpt[i][2] = dpt[i][3] = 0.f; }
-    mma_rows_x_tileT<HD>(st, sK, warp * 16, sQ[buf]);     // S^T  = K Q^T   [16 keys x 64 queries]
-    mma_rows_x_tileT<HD>(dpt, sV, warp * 16, sdO[buf]);   // dP^T = V dO^T
+    mma_rows_x_tileT<HD, WG>(st, sK, warp * 16, sQ[buf]);     // S^T  = K Q^T   [16 keys x 64 queries]
+    mma_rows_x_tileT<HD, WG>(dpt, sV, warp * 16, sdO[buf]);   // dP^T = V dO^T
     float dst[8][4];
     // fast path: the whole 64 x 64 (query, key) tile is in bounds and unmasked
     const bool fast = p.mask == nullptr && k0 + BKV <= p.nk && qb * BQ + BQ <= p.nq &&
@@ -485,8 +538,8 @@ __global__ void __launch_bounds__(THREADS) bwd_dkv_kernel(const Params p_in) {
     uint32_t pa[4][4], dsa[4][4];
     c_to_a(st, pa);
     c_to_a(dst, dsa);
-    mma_p_x_tile<HD>(dv, pa, sdO[buf]);     // dV += P^T dO
-    mma_p_x_tile<HD>(dk, dsa, sQ[buf]);     // dK += dS^T Q
+    mma_p_x_tile<HD, WG>(dv, pa, sdO[buf]);     // dV += P^T dO
+    mma_p_x_tile<HD, WG>(dk, dsa, sQ[buf]);     // dK += dS^T Q
     __syncthreads();
   }
   if (qb0 >= nqb) cp_wait<0>();
@@ -515,35 +568,49 @@ static int validate(const Params& p, int head_dim) {
   return 0;
 }
 
-template <int HD>
-static int launch_fwd(const Params& p, cudaStream_t s) {
-  constexpr int SMEM = 5 * Tile<HD>::BYTES + 128;
+template <int HD, bool WG>
+static int launch_fwd_impl(const Params& p, cudaStream_t s) {
+  constexpr int SMEM = 5 * Tile<HD>::BYTES + 1024;
   static bool done = false;
-  if (!done) { cudaFuncSetAttribute(fwd_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); done = true; }
+  if (!done) { cudaFuncSetAttribute(fwd_kernel<HD, WG>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); done = true; }
   dim3 grid((p.nq + BQ - 1) / BQ, p.heads, p.batch);
-  fwd_kernel<HD><<<grid, THREADS, SMEM, s>>>(p);
+  fwd_kernel<HD, WG><<<grid, THREADS, SMEM, s>>>(p);
   OFK_CHECK_LAUNCH();
   return 0;
 }
-
 template <int HD>
-static int launch_bwd(const Params& p, cudaStream_t s) {
-  constexpr int SMEM = 6 * Tile<HD>::BYTES + 128;
+static int launch_fwd(const Params& p, cudaStream_t s) {
+  if (!ofk_attn_use_wgmma()) return launch_fwd_impl<HD, false>(p, s);
+  if (int rc = launch_fwd_impl<HD, true>(p, s)) return rc;
+  ofk_attn_count_wgmma();
+  return 0;
+}
+
+template <int HD, bool WG>
+static int launch_bwd_impl(const Params& p, cudaStream_t s) {
+  constexpr int SMEM = 6 * Tile<HD>::BYTES + 1024;
   static bool done = false;
   if (!done) {
-    cudaFuncSetAttribute(bwd_dq_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    cudaFuncSetAttribute(bwd_dkv_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
+    cudaFuncSetAttribute(bwd_dq_kernel<HD, WG>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
+    cudaFuncSetAttribute(bwd_dkv_kernel<HD, WG>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
     done = true;
   }
   const long long rows = (long long)p.batch * p.heads * p.nq;
   delta_kernel<HD><<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(p);
   OFK_CHECK_LAUNCH();
   dim3 gq((p.nq + BQ - 1) / BQ, p.heads, p.batch);
-  bwd_dq_kernel<HD><<<gq, THREADS, SMEM, s>>>(p);
+  bwd_dq_kernel<HD, WG><<<gq, THREADS, SMEM, s>>>(p);
   OFK_CHECK_LAUNCH();
   dim3 gk((p.nk + BKV - 1) / BKV, p.heads, p.batch);
-  bwd_dkv_kernel<HD><<<gk, THREADS, SMEM, s>>>(p);
+  bwd_dkv_kernel<HD, WG><<<gk, THREADS, SMEM, s>>>(p);
   OFK_CHECK_LAUNCH();
+  return 0;
+}
+template <int HD>
+static int launch_bwd(const Params& p, cudaStream_t s) {
+  if (!ofk_attn_use_wgmma()) return launch_bwd_impl<HD, false>(p, s);
+  if (int rc = launch_bwd_impl<HD, true>(p, s)) return rc;
+  ofk_attn_count_wgmma();
   return 0;
 }
 
@@ -563,14 +630,6 @@ extern "C" int ofk_attn_dense_fwd(const void* q, const void* k, const void* v, v
   p.scale = scale;
   if (!q || !k || !v || !o) return ofk_set_error(OFK_ERR_ARG, "dense attention: null pointer");
   if (int rc = validate(p, head_dim)) return rc;
-  {
-    ofk::tc::Args a{};
-    a.q = q; a.k = k; a.v = v; a.out = o; a.lse = lse; a.batch = batch; a.heads = heads; a.hd = head_dim; a.nq = nq; a.nk = nk;
-    a.q_bs = q_bstride; a.ldq = ldq; a.k_bs = k_bstride; a.ldk = ldk; a.v_bs = v_bstride; a.ldv = ldv; a.o_bs = o_bstride;
-    a.ldo = ldo; a.scale = scale; a.dense = 1; a.causal = causal; a.mask = mask; a.slopes = slopes; a.pure_causal = pure_causal_flag;
-    a.stream = stream;
-    if (ofk::tc::fwd_supported(a)) return ofk::tc::fwd(a);
-  }
   return head_dim == 64 ? launch_fwd<64>(p, (cudaStream_t)stream) : launch_fwd<128>(p, (cudaStream_t)stream);
 }
 
@@ -580,8 +639,7 @@ extern "C" int ofk_attn_dense_bwd(const void* q, const void* k, const void* v, c
                                   long long ldk, long long v_bstride, long long ldv, long long o_bstride, long long ldo,
                                   long long dq_bstride, long long lddq, long long dk_bstride, long long lddk,
                                   long long dv_bstride, long long lddv, float scale, int causal, const unsigned char* mask,
-                                  const float* slopes, const int* pure_causal_flag, void* workspace,
-                                  long long workspace_bytes, void* stream) {
+                                  const float* slopes, const int* pure_causal_flag, void* stream) {
   using namespace ofk::dense;
   Params p{};
   p.q = (const __nv_bfloat16*)q; p.k = (const __nv_bfloat16*)k; p.v = (const __nv_bfloat16*)v; p.o = (const __nv_bfloat16*)o;
@@ -592,15 +650,5 @@ extern "C" int ofk_attn_dense_bwd(const void* q, const void* k, const void* v, c
   p.dq_bs = dq_bstride; p.lddq = lddq; p.dk_bs = dk_bstride; p.lddk = lddk; p.dv_bs = dv_bstride; p.lddv = lddv; p.scale = scale;
   if (!q || !k || !v || !o || !d_o || !lse || !delta || !dq || !dk || !dv) return ofk_set_error(OFK_ERR_ARG, "dense attention bwd: null pointer");
   if (int rc = validate(p, head_dim)) return rc;
-  {
-    ofk::tc::Args a{};
-    a.q = q; a.k = k; a.v = v; a.o = o; a.d_o = d_o; a.lse = const_cast<float*>(lse); a.delta = delta; a.dq = dq; a.dk = dk;
-    a.dv = dv; a.batch = batch; a.heads = heads; a.hd = head_dim; a.nq = nq; a.nk = nk;
-    a.q_bs = q_bstride; a.ldq = ldq; a.k_bs = k_bstride; a.ldk = ldk; a.v_bs = v_bstride; a.ldv = ldv; a.o_bs = o_bstride;
-    a.ldo = ldo; a.dq_bs = dq_bstride; a.lddq = lddq; a.dk_bs = dk_bstride; a.lddk = lddk; a.dv_bs = dv_bstride; a.lddv = lddv;
-    a.scale = scale; a.dense = 1; a.causal = causal; a.mask = mask; a.slopes = slopes; a.pure_causal = pure_causal_flag;
-    a.workspace = workspace; a.workspace_bytes = workspace_bytes; a.stream = stream;
-    if (ofk::tc::bwd_supported(a)) return ofk::tc::bwd(a);
-  }
   return head_dim == 64 ? launch_bwd<64>(p, (cudaStream_t)stream) : launch_bwd<128>(p, (cudaStream_t)stream);
 }

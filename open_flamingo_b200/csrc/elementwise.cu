@@ -9,10 +9,11 @@
 
 namespace ofk {
 
+constexpr long long MAX_GRID = 132LL * 16;   // 16 blocks per SM of an H100 SXM; also the size of a partials buffer
+
 static inline int grid_for(long long work_items, int threads) {
   long long b = (work_items + threads - 1) / threads;
-  const long long cap = 148LL * 16;
-  if (b > cap) b = cap;
+  if (b > MAX_GRID) b = MAX_GRID;
   if (b < 1) b = 1;
   return (int)b;
 }
@@ -96,7 +97,7 @@ __global__ void cast_f32_bf16_kernel(const float* __restrict__ src, __nv_bfloat1
 // ---- gate backward: dbranch = dout * tanh(g) (bf16); dgate += (1 - tanh(g)^2) * <dout, branch>
 __global__ void __launch_bounds__(256) gate_bwd_kernel(const float* __restrict__ dout, const __nv_bfloat16* __restrict__ branch,
                                                        const float* __restrict__ gate, __nv_bfloat16* __restrict__ dbranch,
-                                                       float* __restrict__ dgate, long long n) {
+                                                       float* __restrict__ part, long long n) {
   __shared__ float s_part[8];
   const float tg = gate ? tanhf(__ldg(gate)) : 1.0f;
   const long long n8 = n / 8;
@@ -112,15 +113,31 @@ __global__ void __launch_bounds__(256) gate_bwd_kernel(const float* __restrict__
     reinterpret_cast<uint4*>(dbranch)[i] = make_uint4(pack_bf16x2(a.x * tg, a.y * tg), pack_bf16x2(a.z * tg, a.w * tg),
                                                       pack_bf16x2(b.x * tg, b.y * tg), pack_bf16x2(b.z * tg, b.w * tg));
   }
-  if (gate && dgate) {
+  if (gate && part) {
     acc = warp_sum(acc);
     if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = acc;
     __syncthreads();
     if (threadIdx.x == 0) {
       float s = 0.f;
       for (int w = 0; w < 8; ++w) s += s_part[w];
-      atomicAdd(dgate, s * (1.0f - tg * tg));
+      part[blockIdx.x] = s * (1.0f - tg * tg);
     }
+  }
+}
+
+// out[0] += sum of part[0, n), one block, in a fixed order: the per-block partials of a grid-wide reduction are
+// combined here instead of with atomics, so the result does not depend on which block finished first.
+__global__ void __launch_bounds__(256) sum_partials_kernel(const float* __restrict__ part, int n, float* __restrict__ out) {
+  __shared__ float s_part[8];
+  float acc = 0.f;
+  for (int i = threadIdx.x; i < n; i += 256) acc += part[i];
+  acc = warp_sum(acc);
+  if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+    for (int w = 0; w < 8; ++w) s += s_part[w];
+    out[0] += s;
   }
 }
 
@@ -213,7 +230,7 @@ __global__ void adamw_kernel(float* __restrict__ p, const float* __restrict__ g,
   }
 }
 
-__global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ x, long long n, float* __restrict__ out) {
+__global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ x, long long n, float* __restrict__ part) {
   __shared__ float s_part[8];
   const long long stride = (long long)gridDim.x * blockDim.x;
   float acc = 0.f;
@@ -224,7 +241,7 @@ __global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ x,
   if (threadIdx.x == 0) {
     float s = 0.f;
     for (int w = 0; w < 8; ++w) s += s_part[w];
-    atomicAdd(out, s);
+    part[blockIdx.x] = s;
   }
 }
 
@@ -267,14 +284,23 @@ extern "C" int ofk_cast_f32_bf16(const float* src, void* dst, long long n, void*
   return 0;
 }
 
+extern "C" long long ofk_reduce_workspace_bytes(void) { return MAX_GRID * (long long)sizeof(float); }
+
 extern "C" int ofk_gate_bwd(const float* dout, const void* branch, const float* gate, void* dbranch, float* dgate,
-                            long long n, void* stream) {
+                            long long n, float* workspace, void* stream) {
   if (!dout || !dbranch || (gate && !branch)) return ofk_set_error(OFK_ERR_ARG, "gate_bwd: null pointer");
+  const bool want_dgate = gate && dgate;
+  if (want_dgate && !workspace) return ofk_set_error(OFK_ERR_ARG, "gate_bwd: dgate needs the reduction workspace");
   if (n <= 0) return 0;
   if (n % 8 != 0) return ofk_set_error(OFK_ERR_ARG, "gate_bwd: n must be a multiple of 8");
-  gate_bwd_kernel<<<grid_for(n / 8, 256), 256, 0, (cudaStream_t)stream>>>(dout, (const __nv_bfloat16*)branch, gate,
-                                                                           (__nv_bfloat16*)dbranch, dgate, n);
+  const int grid = grid_for(n / 8, 256);
+  gate_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(dout, (const __nv_bfloat16*)branch, gate, (__nv_bfloat16*)dbranch,
+                                                          want_dgate ? workspace : nullptr, n);
   OFK_CHECK_LAUNCH();
+  if (want_dgate) {
+    sum_partials_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(workspace, grid, dgate);
+    OFK_CHECK_LAUNCH();
+  }
   return 0;
 }
 
@@ -325,10 +351,13 @@ extern "C" int ofk_adamw(float* param, const float* grad, float* exp_avg, float*
   return 0;
 }
 
-extern "C" int ofk_sumsq(const float* x, long long n, float* out, void* stream) {
-  if (!x || !out) return ofk_set_error(OFK_ERR_ARG, "sumsq: null pointer");
+extern "C" int ofk_sumsq(const float* x, long long n, float* out, float* workspace, void* stream) {
+  if (!x || !out || !workspace) return ofk_set_error(OFK_ERR_ARG, "sumsq: null pointer");
   if (n <= 0) return 0;
-  sumsq_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(x, n, out);
+  const int grid = grid_for(n, 256);
+  sumsq_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, n, workspace);
+  OFK_CHECK_LAUNCH();
+  sum_partials_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(workspace, grid, out);
   OFK_CHECK_LAUNCH();
   return 0;
 }

@@ -79,7 +79,7 @@ __global__ void __launch_bounds__(128) ln_fwd_kernel(const float* __restrict__ x
 // Backward: a 256-thread block walks rows blockIdx.x, +gridDim.x, ...; thread t owns float4 column groups
 // (g*256 + t)*4.  dgamma/dbeta partials stay in registers and are written once per block to the workspace.
 constexpr int LNB_THREADS = 256;
-constexpr int LNB_MAX_BLOCKS = 592;  // 148 SMs x 4 resident blocks
+constexpr int LNB_MAX_BLOCKS = 528;  // 132 SMs x 4 resident blocks
 
 template <int G>
 __global__ void __launch_bounds__(LNB_THREADS) ln_bwd_kernel(
@@ -163,33 +163,25 @@ __global__ void __launch_bounds__(LNB_THREADS) ln_bwd_kernel(
   }
 }
 
-// Column-sum of the per-block partials: 64 columns x 4 row groups per 256-thread block (coalesced 256-byte row
-// segments), the partial rows split over gridDim.y chunks so ~500 blocks share the 2 * D * nblocks floats (a
-// 64-block grid left more than half of the SMs idle and took as long as the backward kernel's own tail);
-// chunk results are combined with one red.global.add per column (dgamma / dbeta accumulate anyway).
-constexpr int LNR_CHUNKS = 8;
+// Column-sum of the per-block partials: 16 columns x 16 row groups per 256-thread block (each row group reads a
+// 64-byte row segment), every column summed by one block in a fixed order, so dgamma / dbeta do not depend on
+// scheduling (no atomics).
 __global__ void __launch_bounds__(256) ln_bwd_reduce_kernel(const float* __restrict__ part, int nblocks, int D,
                                                             float* __restrict__ dgamma, float* __restrict__ dbeta) {
-  __shared__ float s_acc[4][64];
-  const int c = blockIdx.x * 64 + (threadIdx.x & 63);  // over 2*D
-  const int rg = threadIdx.x >> 6;
-  const int per = (nblocks + gridDim.y - 1) / gridDim.y;
-  const int b0 = blockIdx.y * per, b1 = min(nblocks, b0 + per);
-  float s0 = 0.f, s1 = 0.f;
-  if (c < 2 * D) {
-    int b = b0 + rg;
-    for (; b + 4 < b1; b += 8) {
-      s0 += part[(long long)b * 2 * D + c];
-      s1 += part[(long long)(b + 4) * 2 * D + c];
-    }
-    if (b < b1) s0 += part[(long long)b * 2 * D + c];
-  }
-  s_acc[rg][threadIdx.x & 63] = s0 + s1;
+  __shared__ float s_acc[16][16];
+  const int c = blockIdx.x * 16 + (threadIdx.x & 15);  // over 2*D
+  const int rg = threadIdx.x >> 4;
+  float s = 0.f;
+  if (c < 2 * D)
+    for (int b = rg; b < nblocks; b += 16) s += part[(long long)b * 2 * D + c];
+  s_acc[rg][threadIdx.x & 15] = s;
   __syncthreads();
   if (rg == 0 && c < 2 * D) {
-    const float s = (s_acc[0][threadIdx.x] + s_acc[1][threadIdx.x]) + (s_acc[2][threadIdx.x] + s_acc[3][threadIdx.x]);
-    if (c < D) { if (dgamma) atomicAdd(dgamma + c, s); }
-    else if (dbeta) atomicAdd(dbeta + (c - D), s);
+    float t = 0.f;
+#pragma unroll
+    for (int r = 0; r < 16; ++r) t += s_acc[r][threadIdx.x];
+    if (c < D) { if (dgamma) dgamma[c] += t; }
+    else if (dbeta) dbeta[c - D] += t;
   }
 }
 
@@ -242,7 +234,7 @@ extern "C" int ofk_layernorm_bwd(const void* dy, int dy_is_f32, long long lddy, 
     ln_bwd_kernel<4><<<nblocks, LNB_THREADS, 0, s>>>(dy, dy_is_f32, lddy, rows_per_group, group_stride, group_offset, x, ldx, gamma, mean, rstd, rows, D, dx, lddx, dx_add, ldadd, part);
   OFK_CHECK_LAUNCH();
   if (dgamma || dbeta) {
-    ln_bwd_reduce_kernel<<<dim3((2 * D + 63) / 64, nblocks >= 64 ? LNR_CHUNKS : 1), 256, 0, s>>>(part, nblocks, D, dgamma, dbeta);
+    ln_bwd_reduce_kernel<<<(2 * D + 15) / 16, 256, 0, s>>>(part, nblocks, D, dgamma, dbeta);
     OFK_CHECK_LAUNCH();
   }
   return 0;

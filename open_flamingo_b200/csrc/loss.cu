@@ -24,15 +24,11 @@ __device__ __forceinline__ long long row_target(const long long* labels, int T, 
   return labels[row];
 }
 
-// lse[row] (natural log); loss_sum += lse - logit[target]; count += 1 for non-ignored rows.
+// lse[row] (natural log) of every row.
 __global__ void __launch_bounds__(256) ce_fwd_kernel(const void* __restrict__ logits, int is_f32, long long ld, int V,
-                                                     const long long* __restrict__ labels, int T, int shift,
-                                                     long long ignore_index, float* __restrict__ lse,
-                                                     float* __restrict__ loss_sum, float* __restrict__ count) {
+                                                     float* __restrict__ lse) {
   __shared__ float s_m[8], s_l[8];
   const long long row = blockIdx.x;
-  const long long tgt = row_target(labels, T, row, shift);
-  const bool valid = tgt != ignore_index && tgt >= 0 && tgt < V;
   float m = -INFINITY, l = 0.f;
   if (!is_f32 && (V % 8 == 0) && (ld % 8 == 0)) {
     const uint4* p = reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(logits) + row * ld);
@@ -72,10 +68,33 @@ __global__ void __launch_bounds__(256) ce_fwd_kernel(const void* __restrict__ lo
     for (int w = 0; w < 8; ++w) Ls += (s_m[w] == -INFINITY) ? 0.f : s_l[w] * __expf(s_m[w] - M);
     const float L = M + logf(Ls);
     lse[row] = L;
-    if (valid) {
-      atomicAdd(loss_sum, L - load_logit(logits, is_f32, row * ld + tgt));
-      atomicAdd(count, 1.0f);
+  }
+}
+
+// *loss_sum += sum over non-ignored rows of (lse - logit[target]); *count += their number.  One block, fixed order
+// (no atomics), so the loss does not depend on which row finished first.
+__global__ void __launch_bounds__(256) ce_sum_kernel(const void* __restrict__ logits, int is_f32, long long ld, long long rows,
+                                                     int V, const long long* __restrict__ labels, int T, int shift,
+                                                     long long ignore_index, const float* __restrict__ lse,
+                                                     float* __restrict__ loss_sum, float* __restrict__ count) {
+  __shared__ float s_l[8], s_c[8];
+  float acc = 0.f, cnt = 0.f;
+  for (long long row = threadIdx.x; row < rows; row += 256) {
+    const long long tgt = row_target(labels, T, row, shift);
+    if (tgt != ignore_index && tgt >= 0 && tgt < V) {
+      acc += lse[row] - load_logit(logits, is_f32, row * ld + tgt);
+      cnt += 1.0f;
     }
+  }
+  acc = warp_sum(acc);
+  cnt = warp_sum(cnt);
+  if ((threadIdx.x & 31) == 0) { s_l[threadIdx.x >> 5] = acc; s_c[threadIdx.x >> 5] = cnt; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float a = 0.f, b = 0.f;
+    for (int w = 0; w < 8; ++w) { a += s_l[w]; b += s_c[w]; }
+    *loss_sum += a;
+    *count += b;
   }
 }
 
@@ -121,8 +140,10 @@ extern "C" int ofk_ce_fwd(const void* logits, int logits_is_f32, long long ld, l
   if (!logits || !labels || !lse || !loss_sum || !count) return ofk_set_error(OFK_ERR_ARG, "ce_fwd: null pointer");
   if (rows <= 0) return 0;
   if (vocab <= 0 || T <= 0 || rows % T != 0) return ofk_set_error(OFK_ERR_ARG, "ce_fwd: rows must be a multiple of T");
-  ofk::ce_fwd_kernel<<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(logits, logits_is_f32, ld, vocab, labels, T,
-                                                                        shift_labels, ignore_index, lse, loss_sum, count);
+  ofk::ce_fwd_kernel<<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(logits, logits_is_f32, ld, vocab, lse);
+  OFK_CHECK_LAUNCH();
+  ofk::ce_sum_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(logits, logits_is_f32, ld, rows, vocab, labels, T, shift_labels,
+                                                          ignore_index, lse, loss_sum, count);
   OFK_CHECK_LAUNCH();
   return 0;
 }

@@ -5,6 +5,10 @@
 // Records the message returned by ofk_last_error() (thread-local) and returns `code`.
 int ofk_set_error(int code, const char* msg);
 void ofk_count_launch();
+// Attention: true unless the mma.sync kernels were forced (ofk_attn_force_legacy / OFK_ATTN_LEGACY=1); every entry-point
+// call served by the wgmma kernels is counted (ofk_attn_tc_launch_count).
+bool ofk_attn_use_wgmma();
+void ofk_attn_count_wgmma();
 
 #define OFK_CHECK_LAUNCH()                                                        \
   do {                                                                            \
@@ -12,9 +16,3 @@ void ofk_count_launch();
     if (e__ != cudaSuccess) return ofk_set_error(OFK_ERR_CUDA, cudaGetErrorString(e__)); \
     ofk_count_launch();                                                           \
   } while (0)
-
-// Cached cuTensorMapEncodeTiled for a 2-D bf16 row-major tensor [rows, cols] (row stride ld elements), 128B swizzle,
-// box {box_inner (cols), box_outer (rows)}.  Defined in gemm_tcgen05.cu; shared with attention_tc.cu.
-struct CUtensorMap_st;
-int ofk_tensor_map_bf16(const void* ptr, long long ld, int rows, int cols, int box_inner, int box_outer,
-                        struct CUtensorMap_st* out);

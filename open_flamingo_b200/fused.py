@@ -60,35 +60,6 @@ def w16(param):
     return t
 
 
-_SPLIT_CACHE = {}
-
-
-def _wgrad_splits(m, n, k, sms=148):
-    """Split-K factor for a wgrad [m, n] += dy^T x over k tokens (atomic epilogue, so any split is legal).
-    Mirrors the dispatcher in gemm_tcgen05.cu: 256 x 256 tiles on sms/2 SM pairs when m >= 512 and n >= 256, else
-    128 x {128,256} tiles on sms CTAs.  Picks the factor that minimises the number of tile-rounds the persistent
-    grid needs (ceil(tiles * s / units) / s): e.g. the FFN wgrads are 256 tiles on 74 pairs = 3.46 -> 4 rounds
-    unsplit, but 7 half-rounds = 3.5 with s = 2.  A small per-split charge stands for the extra fp32 reductions."""
-    key = (m, n, k)
-    s = _SPLIT_CACHE.get(key)
-    if s is not None:
-        return s
-    if m >= 512 and n >= 256:
-        tiles, units = ((m + 255) // 256) * ((n + 255) // 256), sms // 2
-    else:
-        bn = 256 if (n % 256 == 0 or n > 1024) else 128
-        tiles, units = ((m + 127) // 128) * ((n + bn - 1) // bn), sms
-    kb = (k + 63) // 64
-    best, best_cost = 1, None
-    for cand in range(1, min(16, max(1, kb // 4)) + 1):
-        rounds = -(-tiles * cand // units)
-        cost = rounds / cand + 0.03 * (cand - 1)
-        if best_cost is None or cost < best_cost - 1e-9:
-            best, best_cost = cand, cost
-    _SPLIT_CACHE[key] = best
-    return best
-
-
 class _GradSink:
     """Where a parameter's gradient goes: its `_ofk_grad` bucket view (accumulate, return None) or a fresh tensor."""
 
@@ -112,13 +83,14 @@ class _GradSink:
 
 
 def _wgrad(dy16, x16, sink):
-    """sink += dy^T x   (dy: [R, out], x: [R, in], both bf16, reduction over R; atomic split-K epilogue)."""
+    """sink += dy^T x   (dy: [R, out], x: [R, in], both bf16, reduction over R; accumulating epilogue).  No split-K:
+    split-K partials would land in the gradient in whatever order the CTAs finish, so the gradient would change from
+    run to run in its last bits (and through Adam, by far more at near-zero entries)."""
     buf = sink.buffer()
     if buf is None:
         return
     out_f, in_f = dy16.shape[1], x16.shape[1]
-    ops.gemm(dy16, x16, a_mn=True, b_mn=True, epi=L.EPI_ATOMIC_F32, out=buf.view(out_f, in_f),
-             splits=_wgrad_splits(out_f, in_f, dy16.shape[0]))
+    ops.gemm(dy16, x16, a_mn=True, b_mn=True, epi=L.EPI_ATOMIC_F32, out=buf.view(out_f, in_f))
 
 
 # ------------------------------------------------------------------------------------------ FeedForward
@@ -490,7 +462,7 @@ class PerceiverFoldedLayerFn(torch.autograd.Function):
         if sinks["wkv"].needs or sinks["nm_w"].needs or sinks["nm_b"].needs:
             dweff = torch.zeros((2 * inner, Dv + AUG), device=kv.device, dtype=f32)
             ops.gemm_grouped(dkv, xa, a_mn=True, b_mn=True, epi=L.EPI_ATOMIC_F32, out=dweff, M=2 * inner, N=Dv + AUG,
-                             K=U * v, splits=_wgrad_splits(2 * inner, Dv + AUG, U * v), ak_map=(v, v + n, 0))
+                             K=U * v, ak_map=(v, v + n, 0))
             dw = dweff[:, :Dv]
             if sinks["wkv"].needs:   # d/dW[c, j] of sum_j W[c, j] (x_hat_j gamma_j + beta_j)
                 sinks["wkv"].buffer().addcmul_(dw, nm_w.detach().unsqueeze(0))

@@ -1,9 +1,9 @@
-"""Frozen-LM decoder blocks on the sm_100a kernels (SURVEY.md section 8f, rank 1).
+"""Frozen-LM decoder blocks on the sm_90a kernels (SURVEY.md section 8f, rank 1).
 
 The reference runs the frozen LM's decoder block as ordinary PyTorch (`self.decoder_layer(lang_x, ...)`,
 flamingo_lm.py:63-65).  For the LM family named by BASELINE.json (MPT: HF `MptBlock` = LN -> Wqkv -> causal
 ALiBi attention -> out_proj -> +res -> LN -> up_proj -> GELU(erf) -> down_proj -> +res, no biases) this module
-evaluates the same block with the kernels already used by the gated blocks (tcgen05 GEMMs with fused
+evaluates the same block with the kernels already used by the gated blocks (wgmma GEMMs with fused
 GELU / residual epilogues, LayerNorm, dense attention), forward plus the dgrad-only backward a frozen block
 needs.  Anything else -- other LM families, KV-cache decoding, dropout, clip_qkv, output_attentions -- takes the
 block's own PyTorch forward, exactly as in the reference.

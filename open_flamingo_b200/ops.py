@@ -19,36 +19,18 @@ def _rowmajor_2d(t, name):
         raise ValueError(f"{name} must be 2-D with unit inner stride, got shape {tuple(t.shape)} stride {t.stride()}")
 
 
-_gemm_ws = {}
-
-
-def _gemm_workspace(device):
-    """Scratch for the GEMM tail split (see ofk_gemm_bf16_ws): one buffer per (device, stream) so GEMMs that may
-    overlap never share it.  Allocated through torch's caching allocator, which is also legal while a CUDA graph
-    is being captured (the buffer then lives in the graph's private pool and is kept alive here)."""
-    key = (device, torch.cuda.current_stream(device).cuda_stream)
-    ws = _gemm_ws.get(key)
-    if ws is None:
-        ws = torch.empty(int(L.lib().ofk_gemm_workspace_bytes()), device=device, dtype=torch.uint8)
-        ws[:16384].zero_()   # the flag words (first 16 KiB); they reset themselves after every use
-        _gemm_ws[key] = ws
-    return ws
-
-
 _comm_in_flight = False
 # SMs every persistent GEMM grid leaves to NCCL while gradient-chunk all-reduces are in flight (world > 1 only; 0 = none).
-# Measured at N = 2 inside the captured step (profiles/r02_ddp_timeline_n2.md): with all 148 SMs owned by the GEMM grids the
-# all-reduce kernels are starved (30.8 ms of NCCL kernel time) and the ~60 GEMMs that run beside them take 1.3-1.55 x longer
-# (static tile schedule: the clusters that cannot become resident do their share afterwards) -- 121.1 ms / step; with 16 SMs
-# left free (and NCCL_MAX_CTAS=16, see train.configure_nccl_for_overlap) 117.7 ms.
+# A persistent grid that owns every SM lets the all-reduce kernels in only at GEMM boundaries, so the "overlapped" reduction
+# is serialised behind the GEMMs; 16 free SMs (with NCCL_MAX_CTAS=16, see train.configure_nccl_for_overlap) let it run
+# beside them.  Not measured on H100 (the multi-GPU step needs more than one GPU).
 COMM_RESERVED_SMS = int(os.environ.get("OFK_COMM_RESERVE_SMS", "16"))
 
 
 def set_comm_in_flight(flag):
-    """train.GradBucket brackets the window in which gradient-chunk all-reduces may be running.  Inside it (a) the GEMM
-    tail split is not used: its owner slice spins on flags written by OTHER clusters of the same persistent grid,
-    which assumes all clusters are co-resident -- not guaranteed while NCCL's CTAs hold SMs; (b) the persistent GEMM
-    grids are shrunk by COMM_RESERVED_SMS so the collective's CTAs can run BESIDE the GEMMs instead of between them."""
+    """train.GradBucket brackets the window in which gradient-chunk all-reduces may be running.  Inside it the
+    persistent GEMM grids are shrunk by COMM_RESERVED_SMS so the collective's CTAs can run BESIDE the GEMMs instead of
+    between them."""
     global _comm_in_flight
     flag = bool(flag)
     if flag != _comm_in_flight and COMM_RESERVED_SMS > 0:
@@ -91,13 +73,10 @@ def gemm(a, b, *, a_mn=False, b_mn=False, epi=L.EPI_STORE_BF16, out=None, out2=N
         raise ValueError("gemm bias must be a contiguous float32 vector of length >= N")
     if gate is not None and gate.dtype != f32:
         raise ValueError("gemm gate must be float32")
-    ws = _gemm_workspace(a.device) if (splits == 1 and M >= 512 and N >= 256 and K >= 3072 and not _comm_in_flight) \
-        else None
-    L.check(L.lib().ofk_gemm_bf16_ws(
+    L.check(L.lib().ofk_gemm_bf16(
         epi, int(a_mn), int(b_mn), a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), M, N, K, splits, block_n,
         out.data_ptr(), out.stride(0), L.ptr(out2), 0 if out2 is None else out2.stride(0),
-        L.ptr(aux), 0 if aux is None else aux.stride(0), L.ptr(bias), L.ptr(gate),
-        L.ptr(ws), 0 if ws is None else ws.numel(), L.stream_ptr()))
+        L.ptr(aux), 0 if aux is None else aux.stride(0), L.ptr(bias), L.ptr(gate), L.stream_ptr()))
     return out
 
 
@@ -160,28 +139,14 @@ def _bstride_ld(t, name):
 
 
 def attn_force_legacy(on):
-    """A/B switch: True = always the mma.sync attention kernels, False = TMA + tcgen05 whenever the layout allows
-    (the default).  Returns the previous setting."""
+    """A/B switch: True = the mma.sync attention kernels, False = the wgmma kernels (the default).  Returns the
+    previous setting."""
     return bool(L.lib().ofk_attn_force_legacy(int(bool(on))))
 
 
 def attn_tc_launch_count():
+    """Attention calls (forward or backward) served by the wgmma kernels so far."""
     return int(L.lib().ofk_attn_tc_launch_count())
-
-
-_attn_ws = {}
-
-
-def _attn_workspace(device, nbytes):
-    """fp32 dQ accumulator of the tensor-core attention backward (one per (device, stream), grown on demand)."""
-    if nbytes <= 0:
-        return None
-    key = (device, torch.cuda.current_stream(device).cuda_stream)
-    ws = _attn_ws.get(key)
-    if ws is None or ws.numel() < nbytes:
-        ws = torch.empty(int(nbytes), device=device, dtype=torch.uint8)
-        _attn_ws[key] = ws
-    return ws
 
 
 def attn_fwd(q, k, v, heads, scale, *, mask_mode=L.MASK_NONE, text_time=None, keys_per_media=64, out=None,
@@ -233,12 +198,10 @@ def attn_bwd(q, k, v, o, d_o, lse, heads, scale, *, mask_mode=L.MASK_NONE, text_
     dvb, lddv = _bstride_ld(dv, "dv")
     if text_time is not None:
         text_time = text_time.contiguous()
-    ws = _attn_workspace(q.device, L.lib().ofk_attn_bwd_workspace_bytes(B, heads, 64, nq, nk))
     L.check(L.lib().ofk_attn_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), d_o.data_ptr(), lse.data_ptr(),
                                  delta.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, heads, nq, nk,
                                  qb, ldq, kb, ldk, vb, ldv, ob, ldo, dqb, lddq, dkb, lddk, dvb, lddv, scale, mask_mode,
-                                 L.ptr(text_time), keys_per_media, L.ptr(ws), 0 if ws is None else ws.numel(),
-                                 L.stream_ptr()))
+                                 L.ptr(text_time), keys_per_media, L.stream_ptr()))
     return dq, dk, dv
 
 
@@ -290,14 +253,28 @@ def cast_bf16(src, out=None):
     return out
 
 
+_reduce_ws = {}
+
+
+def _reduce_workspace(device):
+    """Per-block partials of the grid-wide sums (ofk_reduce_workspace_bytes), one buffer per (device, stream)."""
+    key = (device, torch.cuda.current_stream(device).cuda_stream)
+    ws = _reduce_ws.get(key)
+    if ws is None:
+        ws = torch.empty(int(L.lib().ofk_reduce_workspace_bytes()) // 4, device=device, dtype=f32)
+        _reduce_ws[key] = ws
+    return ws
+
+
 def gate_bwd(dout, branch, gate, dgate):
     """dbranch(bf16) = dout * tanh(gate); dgate += (1 - tanh^2) * <dout, branch>.  gate None: plain cast."""
     L.require_cuda(dout)
     if not dout.is_contiguous() or (branch is not None and not branch.is_contiguous()):
         raise ValueError("gate_bwd operands must be contiguous")
     dbranch = torch.empty(dout.shape, device=dout.device, dtype=bf16)
+    ws = _reduce_workspace(dout.device) if (gate is not None and dgate is not None) else None
     L.check(L.lib().ofk_gate_bwd(dout.data_ptr(), L.ptr(branch), L.ptr(gate), dbranch.data_ptr(), L.ptr(dgate),
-                                 dout.numel(), L.stream_ptr()))
+                                 dout.numel(), L.ptr(ws), L.stream_ptr()))
     return dbranch
 
 
@@ -335,7 +312,8 @@ def adamw_(param, grad, exp_avg, exp_avg_sq, w_bf16, lr, beta1, beta2, eps, wd, 
 
 
 def sumsq_(x, out):
-    L.check(L.lib().ofk_sumsq(x.data_ptr(), x.numel(), out.data_ptr(), L.stream_ptr()))
+    L.check(L.lib().ofk_sumsq(x.data_ptr(), x.numel(), out.data_ptr(), _reduce_workspace(x.device).data_ptr(),
+                              L.stream_ptr()))
     return out
 
 
@@ -380,13 +358,11 @@ def attn_dense_bwd(q, k, v, o, d_o, lse, heads, head_dim, scale, *, causal=False
     dqb, lddq = _bstride_ld(dq, "dq")
     dkb, lddk = _bstride_ld(dk, "dk")
     dvb, lddv = _bstride_ld(dv, "dv")
-    ws = _attn_workspace(q.device, L.lib().ofk_attn_bwd_workspace_bytes(B, heads, head_dim, nq, nk))
     L.check(L.lib().ofk_attn_dense_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), d_o.data_ptr(),
                                        lse.data_ptr(), delta.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
                                        B, heads, head_dim, nq, nk, qb, ldq, kb, ldk, vb, ldv, ob, ldo, dqb, lddq, dkb,
                                        lddk, dvb, lddv, scale, int(causal), L.ptr(mask), L.ptr(slopes),
-                                       L.ptr(pure_causal_flag), L.ptr(ws), 0 if ws is None else ws.numel(),
-                                       L.stream_ptr()))
+                                       L.ptr(pure_causal_flag), L.stream_ptr()))
     return dq, dk, dv
 
 

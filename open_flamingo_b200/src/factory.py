@@ -1,8 +1,8 @@
 """create_model_and_transforms -- drop-in for open_flamingo/src/factory.py:11-119 (same signature and return
-triple), building the B200 kernel-backed Flamingo.
+triple), building the H100 kernel-backed Flamingo.
 
-Differences forced by the offline / B200-native setting, none of which change the call signature:
-  * The vision tower is open_flamingo_b200.src.vit.VisionTransformer (sm_100a kernels).  If `open_clip` is
+Differences forced by the offline / H100-native setting, none of which change the call signature:
+  * The vision tower is open_flamingo_b200.src.vit.VisionTransformer (sm_90a kernels).  If `open_clip` is
     importable its pretrained weights and image transform are used (state-dict names are identical); otherwise
     `clip_vision_encoder_path` may be an open_clip model NAME with `clip_vision_encoder_pretrained=None`
     (random init from the built-in config table) or an already-built module exposing `.visual`.
@@ -85,7 +85,7 @@ def _build_vision(clip_vision_encoder_path, clip_vision_encoder_pretrained, cach
         cfg = dict(open_clip.get_model_config(name)["vision_cfg"])
         head_width = cfg.get("head_width", 64)
         if head_width != 64:
-            raise ValueError(f"{name}: head_width {head_width} (open_clip vision_cfg) is not supported -- the sm_100a "
+            raise ValueError(f"{name}: head_width {head_width} (open_clip vision_cfg) is not supported -- the sm_90a "
                              "ViT attention kernel is built for head_dim 64 (ViT-B/L; ViT-H/g/bigG use 80-104)")
         ours = VisionTransformer(image_size=cfg.get("image_size", 224), patch_size=cfg["patch_size"],
                                  width=cfg["width"], layers=cfg["layers"], heads=cfg["width"] // head_width,

@@ -3,8 +3,8 @@ frozen causal LM.
 
 API parity with the reference's open_flamingo/src/flamingo.py (class Flamingo :17-338): same constructor,
 `forward` (:60-122), `generate` (:124-175), `_encode_vision_x` (:177-200), `_condition_media_locations`
-(:303-313), `cache_media` / `uncache_media` (:315-338).  `wrap_fsdp` (:202-301) is out of scope: the B200
-data-parallel path replicates the model (it fits in 180 GB) and all-reduces only the trainable gradients
+(:303-313), `cache_media` / `uncache_media` (:315-338).  `wrap_fsdp` (:202-301) is out of scope: the
+data-parallel path replicates the model (OF-3B training fits one 80 GB H100) and all-reduces only the trainable gradients
 (see open_flamingo_b200/train.py).
 """
 import torch
@@ -123,5 +123,5 @@ class Flamingo(nn.Module):
 
     def wrap_fsdp(self, *args, **kwargs):
         raise NotImplementedError(
-            "FSDP sharding is out of scope for the B200 build: OF-3B/9B fit one 180 GB GPU; use "
+            "FSDP sharding is out of scope for this build: the model is replicated on every GPU; use "
             "open_flamingo_b200.train.FlatTrainer (flat-bucket NCCL all-reduce of the trainable gradients).")

@@ -31,7 +31,7 @@ class FlamingoLayer(nn.Module):
         self.vis_x = None
         self.media_locations = None
         self.use_cached_media = None
-        # recognised frozen decoder blocks (HF MptBlock) are evaluated on the sm_100a kernels; everything else --
+        # recognised frozen decoder blocks (HF MptBlock) are evaluated on the sm_90a kernels; everything else --
         # and every case the fast path declines -- runs the block's own PyTorch forward as in the reference
         self._fast_block = lm_blocks.accelerate(decoder_layer)
         self._pure_causal_flag = None

@@ -1,4 +1,4 @@
-"""Drop-in replacements for the modules of the reference's open_flamingo/src/helpers.py, backed by the sm_100a
+"""Drop-in replacements for the modules of the reference's open_flamingo/src/helpers.py, backed by the sm_90a
 kernels in libofk.so.
 
 Same class names, constructor signatures, parameter names/shapes (state-dict compatible with released
@@ -34,7 +34,7 @@ def FeedForward(dim, mult=4):
 
 def _check_heads(dim_head, heads):
     if dim_head != 64:
-        raise ValueError("the sm_100a attention kernels are specialised for dim_head=64 (the reference default)")
+        raise ValueError("the sm_90a attention kernels are specialised for dim_head=64 (the reference default)")
     if heads < 1:
         raise ValueError("heads must be >= 1")
 

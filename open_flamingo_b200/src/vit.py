@@ -1,4 +1,4 @@
-"""CLIP ViT (ViT-L/14 et al.) forward pass on the sm_100a kernels -- the frozen vision encoder of Flamingo.
+"""CLIP ViT (ViT-L/14 et al.) forward pass on the sm_90a kernels -- the frozen vision encoder of Flamingo.
 
 The reference takes this from open_clip (`open_clip.create_model_and_transforms`, factory.py:42-48; called at
 flamingo.py:195 as `self.vision_encoder(x)[1]` under torch.no_grad).  open_clip is a third-party dependency
@@ -61,7 +61,7 @@ class VisionTransformer(nn.Module):
                  output_dim=768, quick_gelu=True, output_tokens=False):
         super().__init__()
         if width % heads != 0 or width // heads != 64:
-            raise ValueError("the sm_100a attention kernel needs head_dim == 64 (CLIP ViT-B / ViT-L; not ViT-H/g/bigG)")
+            raise ValueError("the sm_90a attention kernel needs head_dim == 64 (CLIP ViT-B / ViT-L; not ViT-H/g/bigG)")
         self.image_size, self.patch_size, self.width, self.heads = image_size, patch_size, width, heads
         self.grid = image_size // patch_size
         self.output_dim = output_dim

@@ -1,6 +1,6 @@
 """Data-parallel training step for the trainable part of Flamingo (resampler + gated cross-attention blocks).
 
-Replaces, for the B200 path, the reference's DDP wrap + clip + AdamW (train/train.py:364-415,
+Replaces, for the H100 path, the reference's DDP wrap + clip + AdamW (train/train.py:364-415,
 train/train_utils.py:94-216):
 
   * GradBucket -- ONE flat fp32 gradient buffer for all trainable hot-path parameters, laid out in backward

@@ -14,7 +14,7 @@ def header_functions():
 
 def test_library_exports_every_declared_symbol():
     import __graft_entry__ as g
-    g.build()  # nvcc cross-compiles for sm_100a without a GPU
+    g.build()  # nvcc cross-compiles for sm_90a without a GPU
     from open_flamingo_b200 import _lib
     lib = ctypes.CDLL(_lib.LIB_PATH)
     declared = header_functions()
@@ -23,7 +23,7 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, name), f"{name} declared in ofk.h but not exported by libofk.so"
     assert sorted(_lib.exported_symbols()) == declared, "ctypes signature table and ofk.h disagree"
     loaded = _lib.lib()
-    assert loaded.ofk_abi_version() == 2
+    assert loaded.ofk_abi_version() == 3
     assert isinstance(_lib.launch_count(), int)
 
 
@@ -72,19 +72,25 @@ def _sass_by_kernel():
     return kernels
 
 
-def test_hot_kernels_are_tcgen05_and_tma_in_the_shipped_binary():
-    """Static proof, on the .so the tests load: the GEMM family and the default attention cores issue tcgen05 MMAs with TMEM
-    accumulators fed by TMA (UTCHMMA / LDTM / UTMALDG), and no mma.sync (HMMA) path hides inside them."""
+def test_hot_kernels_are_wgmma_and_tma_in_the_shipped_binary():
+    """Static proof, on the .so the tests load: every GEMM kernel issues warpgroup MMAs (HGMMA) on operands staged by TMA
+    (UTMALDG), with no mma.sync (HMMA) path inside; the default attention cores issue wgmma and no mma.sync, the
+    reference ones mma.sync."""
     kernels = _sass_by_kernel()
-    assert len(kernels) > 100
-    hot = {k: v for k, v in kernels.items() if re.search(r"attn_fwd2_tc_kernel|attn_bwd_tc_kernel|gemm2_kernel|gemm_kernel", k)}
-    assert sum("attn_fwd2_tc_kernel" in k for k in hot) == 4 and sum("attn_bwd_tc_kernel" in k for k in hot) == 4  # HD x DENSE
-    assert sum("gemm2_kernel" in k for k in hot) >= 10 * 4   # cta_group::2 epilogues x A/B operand layouts
-    for k, ops_ in hot.items():
-        assert "UTCHMMA" in ops_, f"{k}: no tcgen05.mma"
-        assert "LDTM" in ops_, f"{k}: accumulators are not read from TMEM"
+    assert len(kernels) > 40
+    gemms = {k: v for k, v in kernels.items() if "gemm_kernel" in k}
+    assert len(gemms) == 10 * 4   # epilogues x A/B operand layouts
+    for k, ops_ in gemms.items():
+        assert "HGMMA" in ops_, f"{k}: no wgmma"
         assert "UTMALDG" in ops_, f"{k}: operands are not staged by TMA"
-        assert "HMMA" not in ops_, f"{k}: mma.sync inside a tcgen05 kernel"
-    for k, ops_ in hot.items():
-        if "attn_" in k:
-            assert "UTCBAR" in ops_, f"{k}: MMA completion is not tracked by tcgen05.commit -> mbarrier"
+        assert "HMMA" not in ops_, f"{k}: mma.sync inside a wgmma kernel"
+    attn = {k: v for k, v in kernels.items() if re.search(r"attn_fwd_kernel|attn_bwd_dq_kernel|attn_bwd_dkv_kernel|"
+                                                          r"dense\d+fwd_kernel|dense\d+bwd_dq_kernel|dense\d+bwd_dkv_kernel", k)}
+    wg = {k: v for k, v in attn.items() if "Lb1E" in k}      # template flag WG = true: the default path
+    ref = {k: v for k, v in attn.items() if "Lb0E" in k}     # the mma.sync A/B reference
+    assert len(wg) == 3 + 3 * 2 and len(ref) == 3 + 3 * 2, sorted(attn)   # media cores + dense cores for head_dim 64 and 128
+    for k, ops_ in wg.items():
+        assert "HGMMA" in ops_, f"{k}: default attention core without wgmma"
+        assert "HMMA" not in ops_, f"{k}: mma.sync inside a wgmma attention core"
+    for k, ops_ in ref.items():
+        assert "HMMA" in ops_, f"{k}: reference attention core without mma.sync"

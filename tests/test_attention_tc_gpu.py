@@ -1,8 +1,8 @@
-"""GPU: the TMA + tcgen05 attention cores (csrc/attention_tc.cu) are the DEFAULT path of ofk_attn_fwd / ofk_attn_bwd /
-ofk_attn_dense_fwd / ofk_attn_dense_bwd.  Each case is checked three ways: against a plain fp32 torch restatement of
-the reference semantics (helpers.py:190-232 for the media rules; HF MptAttention for the dense rules), against the
-validated mma.sync kernels run on the same inputs (ofk_attn_force_legacy), and by the launch counter that proves the
-tensor-core kernels -- not the legacy ones -- served the default call."""
+"""GPU: the wgmma attention kernels are the DEFAULT path of ofk_attn_fwd / ofk_attn_bwd / ofk_attn_dense_fwd /
+ofk_attn_dense_bwd.  Each case is checked three ways: against a plain fp32 torch restatement of the reference semantics
+(helpers.py:190-232 for the media rules; HF MptAttention for the dense rules), against the mma.sync kernels run on the
+same inputs (ofk_attn_force_legacy), and by the launch counter that proves the wgmma kernels -- not the mma.sync
+ones -- served the default call."""
 import pytest
 import torch
 
@@ -51,10 +51,8 @@ def test_media_attention_tc_vs_reference_and_legacy(ops, case):
             tt[:] = nk // kpm
     n0 = ops.attn_tc_launch_count()
     o, lse, dq, dk, dv = _media_run(ops, q, k, v, d_o, heads, scale, mode, tt, kpm)
-    # forward always; backward too unless the problem has a single half-empty query tile (nq <= 64: the Perceiver
-    # latents / a decode step keep the 64-row mma.sync backward, see attention_tc.cu::bwd_supported)
-    want = 2 if nq > 64 else 1
-    assert ops.attn_tc_launch_count() - n0 == want, "default attention path is not the tcgen05 one"
+    want = 2   # the forward and the backward call
+    assert ops.attn_tc_launch_count() - n0 == want, "default attention path is not the wgmma one"
     prev = ops.attn_force_legacy(True)
     try:
         o2, lse2, dq2, dk2, dv2 = _media_run(ops, q, k, v, d_o, heads, scale, mode, tt, kpm)
@@ -64,11 +62,11 @@ def test_media_attention_tc_vs_reference_and_legacy(ops, case):
     for t in (o, lse, dq, dk, dv):
         assert torch.isfinite(t.float()).all()
     # the two implementations differ only in fp32 summation order and one bf16 rounding of P / dS
-    close(o, o2, 1e-2, "o tc vs mma.sync")
+    close(o, o2, 1e-2, "o wgmma vs mma.sync")
     assert (lse - lse2).abs().max().item() <= 2e-3 * (1 + lse2.abs().max().item())
-    close(dq, dq2, 2e-2, "dq tc vs mma.sync")
-    close(dk, dk2, 2e-2, "dk tc vs mma.sync")
-    close(dv, dv2, 2e-2, "dv tc vs mma.sync")
+    close(dq, dq2, 2e-2, "dq wgmma vs mma.sync")
+    close(dk, dk2, 2e-2, "dk wgmma vs mma.sync")
+    close(dv, dv2, 2e-2, "dv wgmma vs mma.sync")
     # fp32 reference
     qr, kr, vr = (t.float().requires_grad_(True) for t in (q, k, v))
     ref = ref_attention(qr, kr, vr, heads, scale, mode, tt, kpm)
@@ -107,8 +105,8 @@ def test_media_uniform_rows_tc(ops):
 
 
 def test_vit_tail_rows_split(ops):
-    """257 = 2 x 128 + 1 query rows without LSE (the ViT forward): full tiles on the tensor-core kernel, the overhanging
-    row on the 64-row kernel -- same result as the single-kernel path that is taken when an LSE is requested."""
+    """257 = 4 x 64 + 1 query rows (the ViT forward): the forward without an LSE gives the same output as the one
+    that also writes the LSE, and matches fp32 on the overhanging row."""
     torch.manual_seed(19)
     B, heads, n = 3, 16, 257
     qkv = torch.randn(B, n, 3 * heads * 64, device="cuda").to(bf16)
@@ -121,7 +119,7 @@ def test_vit_tail_rows_split(ops):
     torch.cuda.synchronize()
     close(o_split, ref_attention(q, k, v, heads, 0.125, 0, None, 64), 2e-2, "vit split vs fp32")
     assert torch.equal(o_split[:, :256], o_full[:, :256])
-    close(o_split[:, 256:], o_full[:, 256:], 1e-2, "tail row: mma.sync vs tcgen05")
+    close(o_split[:, 256:], o_full[:, 256:], 1e-2, "tail row: without vs with LSE")
 
 
 # ------------------------------------------------------------------ dense (LM self-attention) rules
@@ -192,16 +190,16 @@ def test_dense_attention_tc_vs_reference_and_legacy(ops, case):
 
     n0 = ops.attn_tc_launch_count()
     o, lse, dqkv = run()
-    assert ops.attn_tc_launch_count() - n0 == 2, "default dense attention path is not the tcgen05 one"
+    assert ops.attn_tc_launch_count() - n0 == 2, "default dense attention path is not the wgmma one"
     prev = ops.attn_force_legacy(True)
     try:
         o2, lse2, dqkv2 = run()
     finally:
         ops.attn_force_legacy(prev)
     assert torch.isfinite(o.float()).all() and torch.isfinite(dqkv.float()).all()
-    close(o, o2, 1e-2, "dense o tc vs mma.sync")
+    close(o, o2, 1e-2, "dense o wgmma vs mma.sync")
     assert (lse - lse2).abs().max().item() <= 2e-3 * (1 + lse2.abs().max().item())
-    close(dqkv, dqkv2, 2e-2, "dense dqkv tc vs mma.sync")
+    close(dqkv, dqkv2, 2e-2, "dense dqkv wgmma vs mma.sync")
     qr, kr, vr = (t.float().requires_grad_(True) for t in (q, k, v))
     ref = ref_dense(qr, kr, vr, heads, hd, scale, causal, mask, slopes)
     ref.backward(d_o.float())

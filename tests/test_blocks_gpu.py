@@ -24,7 +24,7 @@ def cmp(got, ref, tol, what):
 def check_gate_grads(what, blk, sd_cpu, x, media, loc, cached, immediate, w, g_ref):
     """The two tanh gates (helpers.py:255-258) get d gate = (1 - tanh^2 g) <dOut, branch>: one scalar that is a sum of
     B*T*D products of mixed sign.  Its error against the fp32 oracle is the projection of the branch's bf16-GEMM rounding
-    noise (relative size eps ~ 5e-3 per element, measured at D = 2048: profiles/r02_gate_grad_noise.md) onto dOut, i.e.
+    noise (relative size eps ~ 5e-3 per element at D = 2048) onto dOut, i.e.
     of order eps * (1 - tanh^2) * ||dOut|| * ||branch|| / sqrt(N) whatever the value of the gradient itself -- so the
     check is against that noise scale (6 sigma, eps = 8e-3) plus 2e-2 of the value, not a percentage of a quantity that
     can cancel to nearly zero.  A second, well-conditioned check follows in the caller (loss = |y|^2 / 2)."""

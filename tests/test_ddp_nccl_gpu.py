@@ -80,7 +80,7 @@ def worker():
     os._exit(0 if ok else 1)
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (NCCL); run with gpurun --gpus 2")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (NCCL)")
 def test_two_micro_batches_two_ranks_nccl():
     s = socket.socket()
     s.bind(("127.0.0.1", 0))

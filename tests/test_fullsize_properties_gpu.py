@@ -1,7 +1,7 @@
 """Size-independent properties checked at BASELINE.json's FULL sizes (configs[1]: OF-3B, 32 x (2 images, 256
 tokens) per GPU), where the fp32 CPU oracle would take minutes per case:
 
-  * tcgen05 GEMM at the FFN shapes: exact integer arithmetic (small-integer operands are exact in bf16 and their
+  * wgmma GEMM at the FFN shapes: exact integer arithmetic (small-integer operands are exact in bf16 and their
     dot products exact in fp32, so the result must equal the integer product BIT FOR BIT), exact power-of-two
     homogeneity, split-K == single pass for exactly representable sums;
   * masked cross-attention at the OF-3B shape: rows of P sum to one (V = 1 gives O = 1), rows before the first

@@ -36,7 +36,7 @@ def test_gemm_majors(ops, L, a_mn, b_mn, shape):
     torch.manual_seed(1)
     a = torch.randn((K, M) if a_mn else (M, K), device="cuda", dtype=bf16)
     b = torch.randn((K, N) if b_mn else (N, K), device="cuda", dtype=bf16)
-    for bn in (128, 256, 512):  # 512 = the 2-CTA (cta_group::2) kernel
+    for bn in (128, 256, 512):  # every accepted tile-width hint
         out = ops.gemm(a, b, a_mn=a_mn, b_mn=b_mn, epi=L.EPI_STORE_F32, block_n=bn)
         A = a.float().t() if a_mn else a.float()
         B = b.float().t() if b_mn else b.float()
@@ -77,7 +77,7 @@ def test_gemm_epilogues(ops, L):
             o = torch.ones(M, N, device="cuda")
             ops.gemm(a, b, epi=L.EPI_ATOMIC_F32, out=o, splits=splits, block_n=bn)
             close(o, acc + 1.0, 2e-3, f"atomic splits={splits} bn={bn}")
-    # the 2-CTA kernel shares the epilogue code; spot-check the fused ones through it as well
+    # the tile-width hint must not change the fused epilogues' results
     close(ops.gemm(a, b, block_n=512), acc.to(bf16), tol, "store_bf16 2cta")
     o = ops.gemm(a, b, epi=L.EPI_GATE_RESID_F32, aux=resid, gate=gate, out2=br, block_n=512)
     close(o, acc.to(bf16).float() * math.tanh(0.7) + resid, tol, "gate_resid 2cta")
@@ -87,10 +87,9 @@ def test_gemm_epilogues(ops, L):
 
 @pytest.mark.parametrize("M,N,K", [(2560, 2048, 4096), (2496, 2048, 3072), (512, 2048, 8192), (8192, 2048, 3072)])
 def test_gemm_tail_split_is_exact_and_epilogue_agnostic(ops, L, M, N, K):
-    """Shapes whose last round of 256 x 256 tiles fills at most half of the 74 SM pairs take the tail split
-    (k-slices of the last tiles exchange fp32 partials through the workspace, ofk_gemm_bf16_ws).  Integer operands
-    make every partial sum exact, so the result must be bit-identical to the unsplit product; the fused epilogues
-    must see the completed sum; repeated launches reuse the self-resetting flags."""
+    """Large-K shapes whose tile count leaves the last round of the persistent grid partly empty.  Integer operands
+    make every partial sum exact, so the result must be bit-identical to the fp32 product whatever the tile hint or
+    operand layout; the fused epilogues must see the completed sum; repeated launches give the same result."""
     g = torch.Generator(device="cuda").manual_seed(21)
     a = torch.randint(-3, 4, (M, K), device="cuda", generator=g).float()
     b = torch.randint(-3, 4, (N, K), device="cuda", generator=g).float()
@@ -103,7 +102,7 @@ def test_gemm_tail_split_is_exact_and_epilogue_agnostic(ops, L, M, N, K):
     a16, b16 = a.to(bf16), b.to(bf16)
     for _ in range(3):
         assert torch.equal(ops.gemm(a16, b16, epi=L.EPI_STORE_F32), ref)
-    assert torch.equal(ops.gemm(a16, b16, epi=L.EPI_STORE_F32, block_n=256), ref)      # 1-CTA kernel: never split
+    assert torch.equal(ops.gemm(a16, b16, epi=L.EPI_STORE_F32, block_n=256), ref)
     assert torch.equal(ops.gemm(a16.t().contiguous(), b16.t().contiguous(), a_mn=True, b_mn=True, epi=L.EPI_STORE_F32), ref)
     resid = torch.randint(-8, 9, (M, N), device="cuda", generator=g).float()
     bias = torch.randint(-8, 9, (N,), device="cuda", generator=g).float()
@@ -118,7 +117,7 @@ def test_gemm_tail_split_is_exact_and_epilogue_agnostic(ops, L, M, N, K):
 
 
 def test_gemm_many_tiles_persistent(ops, L):
-    """More tiles than SMs: exercises the persistent loop, smem-ring and TMEM double-buffer phase wraps."""
+    """More tiles than SMs: exercises the persistent loop and the smem-ring phase wraps."""
     torch.manual_seed(12)
     for (M, N, K, a_mn, b_mn) in [(4096, 4096, 1024, False, False), (4096, 4096, 1024, False, True),
                                   (2048, 4096, 4096, True, True)]:

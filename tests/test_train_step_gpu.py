@@ -138,3 +138,23 @@ def test_checkpoint_resume_continues_the_same_trajectory(tmp_path):
     l_new2 = fwd_bwd(m2, batch)
     assert abs(l_new.item() - l_ref.item()) <= 1e-4 * abs(l_ref.item()), (l_new.item(), l_ref.item())
     assert abs(l_new2.item() - l_ref2.item()) <= 2e-3 * abs(l_ref2.item()), (l_new2.item(), l_ref2.item())
+
+
+def test_training_step_is_bitwise_reproducible():
+    """Two copies of one model, trained on the same batch, end every step with bit-identical loss, gradients and
+    parameters: no reduction in the step may depend on the order in which CTAs finish (Adam would turn such last-bit
+    noise in near-zero gradient entries into parameter changes of up to the learning rate)."""
+    from open_flamingo_b200.train import FlatTrainer
+    m1, batch = build(seed=2)
+    m2 = copy.deepcopy(m1)
+    t1, t2 = FlatTrainer(m1, lr=1e-3), FlatTrainer(m2, lr=1e-3)
+    for step in range(3):
+        losses = []
+        for m, t in ((m1, t1), (m2, t2)):
+            t.zero_grad()
+            losses.append(fwd_bwd(m, batch))
+            t.step()
+        torch.cuda.synchronize()
+        assert torch.equal(losses[0], losses[1]), (step, losses)
+        assert torch.equal(t1.bucket.grads, t2.bucket.grads), f"step {step}: gradients differ"
+        assert torch.equal(t1.bucket.params, t2.bucket.params), f"step {step}: parameters differ"
