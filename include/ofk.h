@@ -62,7 +62,11 @@ long long ofk_launch_count(void);
  *   wgrad    dW += dy^T x    : A=dy [R,out](1), B=x [R,in]   (1), K=R    autograd of the above (ATOMIC_F32)
  *   splits  : split-K factor (ATOMIC_F32 only).  block_n: 0, 128, 256 or 512 -- a tile-width hint; the sm_90a
  *             kernel always uses 128 x 128 tiles, so every accepted value gives the same result.
- * Requirements: N % 16 == 0; operand base pointers 16-byte aligned, lda/ldb % 8 == 0.
+ * Requirements: N % 16 == 0; operand base pointers 16-byte aligned, lda/ldb % 8 == 0.  The epilogue moves its
+ *   operands in 16-byte pieces, so the same holds for every one it uses: `out` 16-byte aligned with ldo % 4 == 0
+ *   (f32 out) or ldo % 8 == 0 (bf16 out); `out2` (bf16) with ldo2 % 8 == 0; `aux` with ldaux % 4 == 0 (f32, the
+ *   RESID epilogues) or % 8 == 0 (bf16, DGELU); `bias` 16-byte aligned.  Violations return OFK_ERR_ALIGN, and every
+ *   argument is checked before the first CUDA call.  K needs no alignment: past K the operands are read as zeros.
  */
 int ofk_gemm_bf16(int epi, int a_mn_major, int b_mn_major, const void* A, long long lda, const void* B,
                   long long ldb, int M, int N, int K, int splits, int block_n, void* out, long long ldo,

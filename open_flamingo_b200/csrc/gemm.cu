@@ -469,8 +469,6 @@ static int get_tensor_map(const void* ptr, long long ld, int rows, int cols, int
   }
   EncodeTiledFn enc = get_encode_fn();
   if (!enc) return ofk_set_error(OFK_ERR_DRIVER, "cuTensorMapEncodeTiled entry point not found");
-  if ((reinterpret_cast<uintptr_t>(ptr) & 15) || ((ld * 2) & 15))
-    return ofk_set_error(OFK_ERR_ALIGN, "GEMM operand must be 16-byte aligned with a 16-byte-multiple row stride");
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
   cuuint32_t box[2] = {(cuuint32_t)box_inner, (cuuint32_t)box_outer};
@@ -563,12 +561,28 @@ static int gemm_impl(int epi, int a_mn_major, int b_mn_major, const void* A, lon
     return ofk_set_error(OFK_ERR_ARG, "GEMM block_n must be 0, 128, 256 or 512");
   if (splits < 1) splits = 1;
   if (splits > 1 && epi != OFK_EPI_ATOMIC_F32) return ofk_set_error(OFK_ERR_ARG, "split-K needs the atomic epilogue");
-  if ((epi == OFK_EPI_BIAS_BF16 || epi == OFK_EPI_BIAS_QGELU_BF16 || epi == OFK_EPI_BIAS_RESID_F32 ||
-       epi == OFK_EPI_BIAS_GELU_BF16) && !bias)
-    return ofk_set_error(OFK_ERR_ARG, "bias epilogue without bias");
+  const bool has_bias = epi == OFK_EPI_BIAS_BF16 || epi == OFK_EPI_BIAS_QGELU_BF16 || epi == OFK_EPI_BIAS_RESID_F32 ||
+                        epi == OFK_EPI_BIAS_GELU_BF16;
+  if (has_bias && !bias) return ofk_set_error(OFK_ERR_ARG, "bias epilogue without bias");
   if ((epi == OFK_EPI_GATE_RESID_F32 || epi == OFK_EPI_BIAS_RESID_F32 || epi == OFK_EPI_DGELU_BF16) && !aux)
     return ofk_set_error(OFK_ERR_ARG, "epilogue needs aux operand");
   if (epi == OFK_EPI_GELU_DUAL && !out2) return ofk_set_error(OFK_ERR_ARG, "GELU_DUAL needs out2");
+  // TMA needs 16-byte-aligned operand bases and row strides; the epilogue moves out / out2 / aux in 16-byte pieces
+  // and reads the bias as float4, so the same holds for every epilogue operand it touches.
+  auto misaligned = [](const void* ptr, long long ld, int elem_bytes) {
+    return (reinterpret_cast<uintptr_t>(ptr) & 15) != 0 || ((ld * elem_bytes) & 15) != 0;
+  };
+  const bool f32_out = epi == OFK_EPI_STORE_F32 || epi == OFK_EPI_ATOMIC_F32 || epi == OFK_EPI_GATE_RESID_F32 ||
+                       epi == OFK_EPI_BIAS_RESID_F32;
+  const bool uses_out2 = epi == OFK_EPI_GELU_DUAL || epi == OFK_EPI_GATE_RESID_F32 || epi == OFK_EPI_BIAS_RESID_F32;
+  const int aux_bytes = (epi == OFK_EPI_GATE_RESID_F32 || epi == OFK_EPI_BIAS_RESID_F32) ? 4 : epi == OFK_EPI_DGELU_BF16 ? 2 : 0;
+  if (misaligned(A, lda, 2) || misaligned(B, ldb, 2))
+    return ofk_set_error(OFK_ERR_ALIGN, "GEMM operand must be 16-byte aligned with a 16-byte-multiple row stride");
+  if (misaligned(out, ldo, f32_out ? 4 : 2) || (uses_out2 && out2 && misaligned(out2, ldo2, 2)) ||
+      (aux_bytes && misaligned(aux, ldaux, aux_bytes)))
+    return ofk_set_error(OFK_ERR_ALIGN, "GEMM out / out2 / aux must be 16-byte aligned with a 16-byte-multiple row stride");
+  if (has_bias && (reinterpret_cast<uintptr_t>(bias) & 15))
+    return ofk_set_error(OFK_ERR_ALIGN, "GEMM bias must be 16-byte aligned");
   if (g_num_sms == 0) {
     int dev = 0;
     cudaGetDevice(&dev);

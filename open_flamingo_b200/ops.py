@@ -67,8 +67,14 @@ def gemm(a, b, *, a_mn=False, b_mn=False, epi=L.EPI_STORE_BF16, out=None, out2=N
         raise ValueError(f"bad out tensor {tuple(out.shape)} {out.dtype} for ({M},{N}) {out_dtype}")
     if out2 is not None:
         _rowmajor_2d(out2, "out2")
+        if out2.dtype != bf16 or out2.shape[0] < M or out2.shape[1] < N:
+            raise ValueError(f"bad out2 tensor {tuple(out2.shape)} {out2.dtype} for ({M},{N}) {bf16}")
     if aux is not None:
         _rowmajor_2d(aux, "aux")
+        aux_dtype = bf16 if epi == L.EPI_DGELU_BF16 else f32
+        if epi in (L.EPI_GATE_RESID_F32, L.EPI_BIAS_RESID_F32, L.EPI_DGELU_BF16) and (
+                aux.dtype != aux_dtype or aux.shape[0] < M or aux.shape[1] < N):
+            raise ValueError(f"bad aux tensor {tuple(aux.shape)} {aux.dtype} for ({M},{N}) {aux_dtype}")
     if bias is not None and (bias.dtype != f32 or bias.numel() < N or not bias.is_contiguous()):
         raise ValueError("gemm bias must be a contiguous float32 vector of length >= N")
     if gate is not None and gate.dtype != f32:
