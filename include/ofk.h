@@ -167,6 +167,26 @@ int ofk_attn_dense_bwd(const void* q, const void* k, const void* v, const void* 
                        long long dv_bstride, long long lddv, float scale, int causal, const unsigned char* mask,
                        const float* slopes, const int* pure_causal_flag, void* stream);
 
+/* Decode attention of the same blocks with a KV cache (HF MptAttention with past_key_values, one new token): split-KV
+ * ("flash-decoding") over the cache, csrc/attention_decode.cu.  Semantics are those of ofk_attn_dense_fwd at nq = 1:
+ *   S = scale * q K^T + slopes[h] * key_index  (slopes NULL = no bias); key_mask[b, key] != 0 sets the score to
+ *   "finfo.min" (a fully masked row attends uniformly); softmax and P.V in fp32, o stored as bf16.
+ *   q: [batch, heads*head_dim] rows (q_bstride), k/v: [batch, nk, heads*head_dim] (shared kv_bstride and row stride
+ *   ldkv -- the K and V column slices of one cache buffer), o like q (o_bstride), key_mask: [batch, >= nk] bytes
+ *   (mask_bstride) or NULL, slopes: [heads] f32 or NULL.
+ *   workspace: caller-owned, >= ofk_attn_decode_workspace_bytes(batch, heads, head_dim, nk) bytes; needs no
+ *   initialisation.  The workspace-size function returns OFK_ERR_ARG for arguments the kernel would reject.
+ * The key split is a pure function of (batch, heads, head_dim, nk, SM count) and partials are merged in a fixed order
+ * without atomics: the output is bitwise identical from launch to launch and does not depend on the cache's capacity.
+ * Requirements: head_dim 64 or 128; batch, heads, nk >= 1 (OFK_ERR_ARG); q, k, v, o, key_mask and workspace 16-byte
+ * aligned, every batch or row stride a multiple of 8 elements (OFK_ERR_ALIGN).  Every argument is checked before the
+ * first CUDA call. */
+long long ofk_attn_decode_workspace_bytes(int batch, int heads, int head_dim, int nk);
+int ofk_attn_decode(const void* q, long long q_bstride, const void* k, const void* v, long long kv_bstride,
+                    long long ldkv, void* o, long long o_bstride, int batch, int heads, int head_dim, int nk,
+                    float scale, const unsigned char* key_mask, long long mask_bstride, const float* slopes,
+                    void* workspace, void* stream);
+
 /* Attention implementation switch, for A/B measurements and for the parity tests that compare the two paths:
  * nonzero = the mma.sync kernels; 0 = the wgmma kernels (the default, unless the environment variable OFK_ATTN_LEGACY=1
  * is set when the library is loaded).  Returns the previous setting.

@@ -62,6 +62,9 @@ _SIGNATURES = {
                                    c_void_p, c_void_p]),
     "ofk_attn_dense_bwd": (c_int, [c_void_p] * 10 + [c_int] * 5 + [c_ll] * 14 + [c_float, c_int, c_void_p, c_void_p,
                                                                               c_void_p, c_void_p]),
+    "ofk_attn_decode_workspace_bytes": (c_ll, [c_int, c_int, c_int, c_int]),
+    "ofk_attn_decode": (c_int, [c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_ll, c_void_p, c_ll, c_int, c_int, c_int,
+                                c_int, c_float, c_void_p, c_ll, c_void_p, c_void_p, c_void_p]),
     "ofk_attn_force_legacy": (c_int, [c_int]),
     "ofk_attn_tc_launch_count": (c_ll, []),
     "ofk_text_time": (c_int, [c_void_p, c_ll, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),

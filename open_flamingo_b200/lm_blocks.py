@@ -5,11 +5,17 @@ flamingo_lm.py:63-65).  For the LM family named by BASELINE.json (MPT: HF `MptBl
 ALiBi attention -> out_proj -> +res -> LN -> up_proj -> GELU(erf) -> down_proj -> +res, no biases) this module
 evaluates the same block with the kernels already used by the gated blocks (wgmma GEMMs with fused
 GELU / residual epilogues, LayerNorm, dense attention), forward plus the dgrad-only backward a frozen block
-needs.  Anything else -- other LM families, KV-cache decoding, dropout, clip_qkv, output_attentions -- takes the
-block's own PyTorch forward, exactly as in the reference.
+needs.
+
+Decoding with a KV cache runs on the kernels too when the cache is a kv_cache.KVCache and no gradient is recorded
+(`no_grad` / `inference_mode`): the K/V projection GEMM writes the new rows straight into the cache buffer, one new
+token attends through the split-KV decode kernel (ops.attn_decode) and a multi-token chunk (prefill, or a chunk after a
+prefix) through the dense kernel over the cached keys.  Anything else -- other LM families, HF's DynamicCache, dropout,
+clip_qkv, output_attentions -- takes the block's own PyTorch forward, exactly as in the reference (a block that declines
+still reads and extends a KVCache through HF's `MptAttention` and `KVCache.update`).
 
 Numerics are those of the block under `torch.autocast(bfloat16)`: fp32 residual stream, fp32 LayerNorm/softmax,
-bf16 GEMM operands.
+bf16 GEMM operands, bf16 K/V cache.
 """
 import weakref
 
@@ -18,6 +24,7 @@ import torch
 from . import _lib as L
 from . import ops
 from .fused import w16
+from .kv_cache import KVCache
 
 bf16 = torch.bfloat16
 f32 = torch.float32
@@ -25,7 +32,9 @@ f32 = torch.float32
 ENABLED = True  # module-level switch (bench.py --lm eager turns it off to time the reference's PyTorch LM path)
 
 _zero_bias = {}
-_mask_cache = [None, None]  # (weakref to HF's [B,1,T,T] bool mask, its contiguous [B,T,T] byte view) -- one per forward
+# (weakref to HF's [B,1,T,nk] bool mask, its byte form for the kernels, whether that is the decode form) -- converted
+# once per forward and shared by every block
+_mask_cache = [None, None, None]
 
 
 def _zeros(n, device):
@@ -37,6 +46,53 @@ def _zeros(n, device):
     return t
 
 
+def _block_tail(x2d, o, eps, wout, n2_w, wup, wdown):
+    """The block after its attention core: out-proj + residual -> LayerNorm -> up-proj GELU -> down-proj + residual.
+    x2d: [R, D] f32 block input, o: [R, D] bf16 attention output.  Returns (out, x1, mean2, rstd2, z); the last four
+    are what the backward needs."""
+    R, D = x2d.shape
+    x1 = ops.gemm(o, w16(wout), epi=L.EPI_GATE_RESID_F32, aux=x2d)                 # + residual
+    x1n, mean2, rstd2 = ops.layernorm_fwd(x1, n2_w, _zeros(D, x2d.device), eps)
+    z = torch.empty((R, wup.shape[0]), device=x2d.device, dtype=bf16)
+    h = torch.empty((R, wup.shape[0]), device=x2d.device, dtype=bf16)
+    ops.gemm(x1n, w16(wup), epi=L.EPI_GELU_DUAL, out=z, out2=h)
+    del x1n
+    out = ops.gemm(h, w16(wdown), epi=L.EPI_GATE_RESID_F32, aux=x1)                # + residual
+    return out, x1, mean2, rstd2, z
+
+
+def cached_block_forward(x, layer, mask, pure_flag, slopes, heads, eps, n1_w, wqkv, wout, n2_w, wup, wdown):
+    """Inference forward of one block that appends its nq new tokens to `layer` (a kv_cache.KVCacheLayer) and attends
+    over everything cached.  x: [B, nq, D] f32.  mask: nq == 1: [B, >= nk] bytes (key padding, row stride a multiple
+    of 8); nq > 1: [B, nq, nk] bytes; None = causal only.  Returns [B, nq, D] f32."""
+    B, nq, D = x.shape
+    R = B * nq
+    hd = D // heads
+    x2d = x.reshape(R, D)
+    if not x2d.is_contiguous():
+        x2d = x2d.contiguous()
+    xn, _, _ = ops.layernorm_fwd(x2d, n1_w, _zeros(D, x.device), eps, want_stats=False)
+    w = w16(wqkv)
+    q = ops.gemm(xn, w[:D])                                                         # [R, D]
+    if not layer.is_initialized:
+        layer.init_storage(B, heads, hd, bf16, x.device)
+    past = layer.length
+    buf = layer.reserve(nq)
+    cap = buf.shape[1]
+    # K and V rows land in cache rows [past, past + nq) of every batch entry: logical row b*nq + t -> b*cap + past + t
+    ops.gemm_grouped(xn, w[D:], out=buf.view(B * cap, 2 * D), M=R, N=2 * D, K=D, out_map=(nq, cap, past))
+    del xn
+    layer.length = past + nq
+    k, v = layer.kv_views()
+    scale = float(hd ** -0.5)
+    if nq == 1:
+        o = ops.attn_decode(q, k, v, heads, hd, scale, key_mask=mask, slopes=slopes)
+    else:
+        o, _ = ops.attn_dense_fwd(q.view(B, nq, D), k, v, heads, hd, scale, causal=mask is None, mask=mask,
+                                  slopes=slopes, pure_causal_flag=pure_flag, want_lse=False)
+    return _block_tail(x2d, o.view(R, D), eps, wout, n2_w, wup, wdown)[0].view(B, nq, D)
+
+
 class FrozenMptBlockFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, mask, pure_flag, slopes, heads, eps, n1_w, wqkv, wout, n2_w, wup, wdown):
@@ -46,22 +102,14 @@ class FrozenMptBlockFn(torch.autograd.Function):
         x2d = x.reshape(R, D)
         if not x2d.is_contiguous():
             x2d = x2d.contiguous()
-        zb = _zeros(D, x.device)
-        xn, mean1, rstd1 = ops.layernorm_fwd(x2d, n1_w, zb, eps)
+        xn, mean1, rstd1 = ops.layernorm_fwd(x2d, n1_w, _zeros(D, x.device), eps)
         qkv = ops.gemm(xn, w16(wqkv))                                               # [R, 3D]
         del xn
         q3 = qkv.view(B, T, 3 * D)
         scale = float(hd ** -0.5)
         o, lse = ops.attn_dense_fwd(q3[..., :D], q3[..., D:2 * D], q3[..., 2 * D:], heads, hd, scale,
                                     causal=mask is None, mask=mask, slopes=slopes, pure_causal_flag=pure_flag)
-        x1 = ops.gemm(o.view(R, D), w16(wout), epi=L.EPI_GATE_RESID_F32, aux=x2d)   # + residual
-        x1n, mean2, rstd2 = ops.layernorm_fwd(x1, n2_w, zb, eps)
-        z = torch.empty((R, wup.shape[0]), device=x.device, dtype=bf16)
-        h = torch.empty((R, wup.shape[0]), device=x.device, dtype=bf16)
-        ops.gemm(x1n, w16(wup), epi=L.EPI_GELU_DUAL, out=z, out2=h)
-        del x1n
-        out = ops.gemm(h, w16(wdown), epi=L.EPI_GATE_RESID_F32, aux=x1)             # + residual
-        del h
+        out, x1, mean2, rstd2, z = _block_tail(x2d, o.view(R, D), eps, wout, n2_w, wup, wdown)
         ctx.save_for_backward(x2d, mean1, rstd1, qkv, o, lse, x1, mean2, rstd2, z, n1_w, wqkv, wout, n2_w, wup,
                               wdown, slopes, mask if mask is not None else x2d.new_empty(0),
                               pure_flag if pure_flag is not None else x2d.new_empty(0))
@@ -117,12 +165,11 @@ class FastMptBlock:
         self.block = block
         self._slopes = None
 
-    def applicable(self, hidden_states, position_bias, attention_mask, layer_past, use_cache, output_attentions):
+    def supported(self, hidden_states, position_bias, output_attentions):
+        """The block and call are ones the kernels evaluate, whatever the cache."""
         b = self.block
-        if not ENABLED or not hidden_states.is_cuda or layer_past is not None or output_attentions:
+        if not ENABLED or not hidden_states.is_cuda or output_attentions:
             return False
-        if use_cache:
-            return False   # a caller that wants a `present` back (tuple-cache HF versions) gets the block's own forward
         a = b.attn
         if getattr(a, "clip_qkv", None) or (b.training and (a.attn_dropout_p > 0 or b.dropout_rate > 0 or
                                                             b.ffn.hidden_dropout > 0)):
@@ -140,9 +187,38 @@ class FastMptBlock:
             return False
         return True
 
+    def applicable(self, hidden_states, position_bias, attention_mask, layer_past, use_cache, output_attentions):
+        """The uncached path (FrozenMptBlockFn, forward and backward)."""
+        if layer_past is not None or use_cache:
+            return False   # a cache other than KVCache, or a caller that wants a `present` back: the block's own forward
+        return self.supported(hidden_states, position_bias, output_attentions)
+
+    def cache_layer(self, hidden_states, position_bias, layer_past, output_attentions):
+        """The KVCacheLayer the cached path appends to, or None when that path does not apply: it needs a KVCache whose
+        layer is empty or holds bf16 storage on this device for this batch, and no gradient being recorded."""
+        if not isinstance(layer_past, KVCache) or torch.is_grad_enabled():
+            return None
+        if not self.supported(hidden_states, position_bias, output_attentions):
+            return None
+        a = self.block.attn
+        if a.layer_idx is None or not 0 <= a.layer_idx < len(layer_past.layers):
+            return None
+        layer = layer_past.layers[a.layer_idx]
+        if layer.is_initialized and (layer.buf.dtype != bf16 or layer.buf.device != hidden_states.device or
+                                     layer.buf.shape[0] != hidden_states.shape[0] or layer.heads != a.n_heads or
+                                     layer.head_dim != a.head_dim):
+            return None
+        return layer
+
     def __call__(self, hidden_states, position_bias=None, attention_mask=None, layer_past=None, use_cache=False,
                  output_attentions=False, pure_causal_flag=None, **kwargs):
-        if not self.applicable(hidden_states, position_bias, attention_mask, layer_past, use_cache, output_attentions):
+        layer = None
+        if layer_past is not None or use_cache:
+            layer = self.cache_layer(hidden_states, position_bias, layer_past, output_attentions)
+            if layer is None:
+                return None
+        elif not self.applicable(hidden_states, position_bias, attention_mask, layer_past, use_cache,
+                                 output_attentions):
             return None
         b = self.block
         a = b.attn
@@ -151,20 +227,32 @@ class FastMptBlock:
             self._slopes = _alibi_slopes(position_bias)
             if self._slopes is None:
                 return None
+        nk = T if layer is None else layer.length + T
+        decode = layer is not None and T == 1
         mask = None
         if attention_mask is not None:
             m = attention_mask
-            if m.dtype != torch.bool or m.dim() != 4 or m.shape[1] != 1 or m.shape[2] != T or m.shape[3] != T:
+            if m.dtype != torch.bool or m.dim() != 4 or m.shape[0] not in (1, B) or m.shape[1] != 1 or \
+                    m.shape[2] != T or m.shape[3] != nk:
                 return None
             ref = _mask_cache[0]
-            if ref is not None and ref() is m and _mask_cache[1].shape[0] == B:
+            if ref is not None and ref() is m and _mask_cache[1].shape[0] == B and _mask_cache[2] == decode:
                 mask = _mask_cache[1]
             else:
-                mask = m.expand(B, 1, T, T).reshape(B, T, T).contiguous()
-                _mask_cache[0], _mask_cache[1] = weakref.ref(m), mask
+                if decode:   # key padding only, rows padded to a multiple of 8 bytes for the decode kernel
+                    mask = torch.zeros((B, -(-nk // 8) * 8), dtype=torch.uint8, device=m.device)
+                    mask[:, :nk].copy_(m.expand(B, 1, 1, nk).reshape(B, nk))
+                else:
+                    mask = m.expand(B, 1, T, nk).reshape(B, T, nk).contiguous()
+                _mask_cache[0], _mask_cache[1], _mask_cache[2] = weakref.ref(m), mask, decode
         x = hidden_states if hidden_states.dtype == f32 else hidden_states.float()
-        out = FrozenMptBlockFn.apply(x, mask, pure_causal_flag if mask is not None else None, self._slopes, a.n_heads, b.norm_1.eps, b.norm_1.weight, a.Wqkv.weight,
-                                     a.out_proj.weight, b.norm_2.weight, b.ffn.up_proj.weight, b.ffn.down_proj.weight)
+        weights = (b.norm_1.weight, a.Wqkv.weight, a.out_proj.weight, b.norm_2.weight, b.ffn.up_proj.weight,
+                   b.ffn.down_proj.weight)
+        flag = pure_causal_flag if mask is not None else None
+        if layer is not None:
+            out = cached_block_forward(x, layer, mask, flag, self._slopes, a.n_heads, b.norm_1.eps, *weights)
+        else:
+            out = FrozenMptBlockFn.apply(x, mask, flag, self._slopes, a.n_heads, b.norm_1.eps, *weights)
         if out.dtype != hidden_states.dtype:
             out = out.to(hidden_states.dtype)
         return out, None

@@ -343,6 +343,56 @@ def attn_dense_fwd(q, k, v, heads, head_dim, scale, *, causal=False, mask=None, 
     return out, lse
 
 
+_decode_ws = {}
+
+
+def _decode_workspace(device, B, heads, head_dim, nk):
+    """Split partials of ofk_attn_decode, one grow-only buffer per (device, stream)."""
+    need = int(L.lib().ofk_attn_decode_workspace_bytes(B, heads, head_dim, nk))
+    if need < 0:
+        raise ValueError(f"attn_decode: unsupported problem (batch {B}, heads {heads}, head_dim {head_dim}, nk {nk})")
+    key = (device, torch.cuda.current_stream(device).cuda_stream)
+    ws = _decode_ws.get(key)
+    if ws is None or ws.numel() * 4 < need:
+        ws = torch.empty((need + 3) // 4, device=device, dtype=f32)
+        _decode_ws[key] = ws
+    return ws
+
+
+def attn_decode(q, k, v, heads, head_dim, scale, *, key_mask=None, slopes=None, out=None):
+    """Decode attention (one query row per batch entry and head) over the first nk rows of a K/V cache.
+    q: [B, heads*head_dim] with unit inner stride (e.g. a column slice of a qkv row); k/v: [B, nk, heads*head_dim] views
+    with the same strides (the K and V column slices of one cache buffer); key_mask: [B, >= nk] 1-byte tensor
+    (nonzero = masked) with unit inner stride; slopes: [heads] f32 ALiBi slopes.  Returns o [B, heads*head_dim] bf16."""
+    L.require_cuda(q, k, v, key_mask, slopes)
+    if q.dtype != bf16 or k.dtype != bf16 or v.dtype != bf16:
+        raise ValueError("attention operands must be bfloat16")
+    inner = heads * head_dim
+    if q.dim() != 2 or q.shape[1] != inner or q.stride(1) != 1:
+        raise ValueError(f"q must be [B, {inner}] with unit inner stride, got {tuple(q.shape)} stride {q.stride()}")
+    B = q.shape[0]
+    if k.dim() != 3 or tuple(k.shape) != tuple(v.shape) or k.shape[0] != B or k.shape[2] != inner or \
+            k.stride(2) != 1 or k.stride() != v.stride():
+        raise ValueError(f"k/v must be [B, nk, {inner}] views with equal strides and unit inner stride, got "
+                         f"{tuple(k.shape)} {k.stride()} / {tuple(v.shape)} {v.stride()}")
+    nk = k.shape[1]
+    if key_mask is not None and (key_mask.dim() != 2 or key_mask.shape[0] != B or key_mask.shape[1] < nk or
+                                 key_mask.element_size() != 1 or key_mask.stride(1) != 1):
+        raise ValueError(f"key_mask must be a 1-byte [B, >= {nk}] tensor with unit inner stride")
+    if slopes is not None and (slopes.dtype != f32 or slopes.numel() < heads or not slopes.is_contiguous()):
+        raise ValueError("slopes must be a contiguous float32 vector of length >= heads")
+    if out is None:
+        out = torch.empty((B, inner), device=q.device, dtype=bf16)
+    elif out.dtype != bf16 or out.dim() != 2 or tuple(out.shape) != (B, inner) or out.stride(1) != 1:
+        raise ValueError(f"out must be a bf16 [B, {inner}] tensor with unit inner stride")
+    ws = _decode_workspace(q.device, B, heads, head_dim, nk)
+    L.check(L.lib().ofk_attn_decode(q.data_ptr(), q.stride(0), k.data_ptr(), v.data_ptr(), k.stride(0), k.stride(1),
+                                    out.data_ptr(), out.stride(0), B, heads, head_dim, nk, scale, L.ptr(key_mask),
+                                    0 if key_mask is None else key_mask.stride(0), L.ptr(slopes), ws.data_ptr(),
+                                    L.stream_ptr()))
+    return out
+
+
 def attn_dense_bwd(q, k, v, o, d_o, lse, heads, head_dim, scale, *, causal=False, mask=None, slopes=None,
                    pure_causal_flag=None, dq=None, dk=None, dv=None):
     L.require_cuda(q, k, v, o, d_o)

@@ -77,7 +77,9 @@ class Flamingo(nn.Module):
     # ------------------------------------------------------------------ generate
     def generate(self, vision_x: torch.Tensor, lang_x: torch.Tensor, attention_mask: torch.Tensor = None, **kwargs):
         """HF generate() conditioned on images; kwargs are forwarded (max_new_tokens, num_beams, ...).
-        Returns lang_x with the generated tokens appended."""
+        Returns lang_x with the generated tokens appended.  When generation uses a cache (`use_cache=True`) under
+        bf16 autocast, the frozen MPT blocks decode on the kernels through a kv_cache.KVCache (see
+        FlamingoLMMixin.make_kv_cache)."""
         num_beams = kwargs.pop("num_beams", 1)
         if num_beams > 1:
             vision_x = vision_x.repeat_interleave(num_beams, dim=0)
@@ -86,6 +88,10 @@ class Flamingo(nn.Module):
         try:
             self._encode_vision_x(vision_x=vision_x)
             eos_token_id = kwargs.pop("eos_token_id", self.eoc_token_id)
+            if kwargs.get("past_key_values") is None and kwargs.get("use_cache", lm.generation_config.use_cache):
+                cache = lm.make_kv_cache()   # bf16 decoding on the kernels; None keeps HF's DynamicCache
+                if cache is not None:
+                    kwargs["past_key_values"] = cache
             output = lm.generate(input_ids=lang_x, attention_mask=attention_mask, eos_token_id=eos_token_id,
                                  num_beams=num_beams, **kwargs)
         finally:

@@ -12,6 +12,7 @@ import torch
 import torch.nn as nn
 
 from .. import lm_blocks
+from ..kv_cache import KVCache
 from .helpers import GatedCrossAttentionBlock
 from .utils import getattr_recursive, setattr_recursive
 
@@ -116,6 +117,10 @@ class FlamingoLMMixin(nn.Module):
         the attention kernel and the capture-safe 4-D mask (see below)."""
         if not getattr(self, "initialized_flamingo", False):
             raise ValueError("Flamingo layers are not initialized. Please call `init_flamingo` first.")
+        if kwargs.get("use_cache") and kwargs.get("past_key_values") is None:
+            cache = self.make_kv_cache()   # a cached prefix (rank classification): decode its continuation on the kernels
+            if cache is not None:
+                kwargs["past_key_values"] = cache
         media_locations = input_ids == self.media_token_id
         # HF generate() feeds one token at a time after the prompt; such calls carry no <image> token and must
         # keep attending to the last cached image (flamingo_lm.py:137-146).
@@ -144,6 +149,21 @@ class FlamingoLMMixin(nn.Module):
                 m4 = m4 | (attention_mask == 0).view(input_ids.shape[0], 1, 1, T)
             attention_mask = m4.contiguous()
         return super().forward(input_ids=input_ids, attention_mask=attention_mask, **kwargs)
+
+    def make_kv_cache(self):
+        """A kv_cache.KVCache for decoding this LM on the kernels, or None where HF's own cache is kept: it is made only
+        on CUDA, under `torch.autocast("cuda", dtype=torch.bfloat16)` (the caller asked for bf16 numerics; the cache
+        stores bf16), with lm_blocks.ENABLED, and when every decoder block is a recognised MPT block.  In fp32 every
+        path stays HF's."""
+        if not lm_blocks.ENABLED or not torch.is_autocast_enabled("cuda") or \
+                torch.get_autocast_dtype("cuda") != torch.bfloat16:
+            return None
+        layers = self._get_decoder_layers()
+        if not all(isinstance(layer, FlamingoLayer) and layer._fast_block is not None for layer in layers):
+            return None
+        if not self.get_input_embeddings().weight.is_cuda:
+            return None
+        return KVCache(len(layers))
 
     def is_conditioned(self) -> bool:
         """All layers hold vis_x and media_locations (flamingo_lm.py:157-159)."""

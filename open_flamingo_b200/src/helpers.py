@@ -139,13 +139,18 @@ class MediaContext:
     __slots__ = ("media_ref", "media_version", "loc_ref", "cached", "t_txt", "media16", "text_time", "kv")
 
     def matches(self, media, media_locations, use_cached_media, t_txt):
-        if self.media_ref() is not media or self.media_version != media._version:
+        if self.media_ref() is not media or self.media_version != _tensor_version(media):
             return False
         if (self.loc_ref is None) != (media_locations is None):
             return False
         if self.loc_ref is not None and self.loc_ref() is not media_locations:
             return False
         return self.cached == bool(use_cached_media) and self.t_txt == t_txt
+
+
+def _tensor_version(t):
+    """In-place version counter; None for a tensor made under torch.inference_mode, which has none."""
+    return None if t.is_inference() else t._version
 
 
 _shared_media_ctx = None  # one entry: all gated blocks of a forward pass see the same (media, media_locations) objects
@@ -160,7 +165,7 @@ def get_media_context(media, media_locations, use_cached_media, t_txt):
     ctx = MediaContext()
     B, T_img, n, Dv = media.shape
     ctx.media_ref = weakref.ref(media)
-    ctx.media_version = media._version
+    ctx.media_version = _tensor_version(media)
     ctx.loc_ref = None if media_locations is None else weakref.ref(media_locations)
     ctx.cached = bool(use_cached_media)
     ctx.t_txt = t_txt
@@ -169,7 +174,7 @@ def get_media_context(media, media_locations, use_cached_media, t_txt):
     # per-layer media K/V for inference: survives across decode steps of one generate() call because the media
     # tensor object (and hence media16) is unchanged while only (media_locations, t_txt) vary
     prev = _shared_media_ctx
-    same_media = prev is not None and prev.media_ref() is media and prev.media_version == media._version
+    same_media = prev is not None and prev.media_ref() is media and prev.media_version == _tensor_version(media)
     ctx.kv = prev.kv if same_media else {}
     if same_media:
         ctx.media16 = prev.media16
