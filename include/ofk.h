@@ -60,8 +60,8 @@ long long ofk_launch_count(void);
  *   forward  y = x W^T       : A=x [R,in]  (0), B=W [out,in] (0)         nn.Linear (helpers.py:18-21,35-37,153-155)
  *   dgrad    dx = dy W       : A=dy [R,out](0), B=W [out,in] (1), K=out  autograd of the above
  *   wgrad    dW += dy^T x    : A=dy [R,out](1), B=x [R,in]   (1), K=R    autograd of the above (ATOMIC_F32)
- *   splits  : split-K factor (ATOMIC_F32 only).  block_n: 0, 128, 256 or 512 -- a tile-width hint; the sm_90a
- *             kernel always uses 128 x 128 tiles, so every accepted value gives the same result.
+ *   splits  : split-K factor (ATOMIC_F32 only).  block_n: 0, 128, 256 or 512 -- a tile-width hint, ignored: the
+ *             sm_90a kernel picks 128 x 128 or 128 x 256 tiles from the problem's size, and both give the same bits.
  * Requirements: N % 16 == 0; operand base pointers 16-byte aligned, lda/ldb % 8 == 0.  The epilogue moves its
  *   operands in 16-byte pieces, so the same holds for every one it uses: `out` 16-byte aligned with ldo % 4 == 0
  *   (f32 out) or ldo % 8 == 0 (bf16 out); `out2` (bf16) with ldo2 % 8 == 0; `aux` with ldaux % 4 == 0 (f32, the

@@ -1,6 +1,14 @@
 // bf16 x bf16 -> fp32 GEMM for sm_90a: TMA-staged operands (128B swizzle), wgmma with the accumulator in registers,
 // a warp-specialised persistent CTA (one producer warp, two consumer warpgroups), fused epilogues.
 //
+// Two tile shapes, chosen per launch from the problem's size (launch()):
+//   wide  : 128 x 256 tiles on 2-CTA clusters.  The two CTAs compute vertically adjacent m-tiles of the same n-tile;
+//           each loads its own A and one half of the shared B panel, multicast into both CTAs' shared memory, so a
+//           k-block costs 32 KiB of L2 reads for 4.2 MFLOP per CTA (128 x 128 tiles: 32 KiB for 2.1 MFLOP).
+//   narrow: 128 x 128 tiles, no cluster, for problems whose wide work items would not fill the GPU once (the small-M
+//           GEMMs of decoding, some Perceiver shapes).
+// Both reduce every output element over k in the same order, so the choice never changes a bit of the result.
+//
 //   out[m, n] = epilogue( sum_k A(m, k) * B(n, k) )
 //
 // Operand storage ("major"):
@@ -21,6 +29,7 @@
 #include <stdlib.h>
 
 #include <mutex>
+#include <type_traits>
 #include <unordered_map>
 
 #include "ofk_internal.h"
@@ -29,12 +38,13 @@
 namespace ofk {
 
 constexpr int BM = 128;       // two consumer warpgroups x wgmma M = 64
-constexpr int BN = 128;       // wgmma N
+constexpr int BN = 128;       // narrow tile width; also the B rows one CTA loads per k-block in either shape
+constexpr int BN_WIDE = 256;  // wide tile width (wgmma N = 256)
+constexpr int CLUSTER = 2;    // CTAs per cluster in the wide shape
 constexpr int BK = 64;        // one 128-byte swizzle atom of bf16
 constexpr int WGMMA_K = 16;   // fixed for 16-bit inputs
-constexpr int STAGES = 4;     // TMA ring depth (32 KiB per stage)
 // Warp roles: warpgroup 0 = producer (warp 0 lane 0 issues every TMA load; the other warps only take part in set-up),
-// warpgroups 1 and 2 = consumers, each owning 64 accumulator rows of the 128 x 128 tile through mainloop and epilogue.
+// warpgroups 1 and 2 = consumers, each owning 64 accumulator rows of the tile through mainloop and epilogue.
 constexpr int NUM_CONSUMER_WG = 2;
 constexpr int NUM_EPI_WARPS = 4 * NUM_CONSUMER_WG;
 constexpr int NUM_THREADS = 128 * (1 + NUM_CONSUMER_WG);
@@ -58,13 +68,15 @@ struct GemmParams {
   // helpers.py:53); `ak_*` does the same for the REDUCTION rows of an MN-major A operand (wgrad over one half).
   int out_rpg, out_gs, out_go;
   int ak_rpg, ak_gs, ak_go;
+  int wide;          // 1: 128 x 256 tiles on 2-CTA clusters sharing B (launched with a cluster); 0: 128 x 128 tiles
 };
 __device__ __forceinline__ long long map_rows(long long r, int rpg, int gs, int go) {
   return rpg > 0 ? (r / rpg) * gs + go + r % rpg : r;
 }
 
-// Work item -> (m tile, n tile, k split).  Within a split, tiles are walked in groups of GROUP_M m-tiles by all
-// n-tiles, m fastest, so the tiles in flight share GROUP_M row panels of A and a few column panels of B through L2.
+// Work item -> (m unit, n tile, k split); an m unit is an m-tile (narrow) or a cluster's pair of m-tiles (wide).
+// Within a split, tiles are walked in groups of GROUP_M m units by all n-tiles, m fastest, so the tiles in flight
+// share GROUP_M row panels of A and a few column panels of B through L2.
 __device__ __forceinline__ void work_to_tile(int w, int m_tiles, int n_tiles, int& mt, int& nt, int& ks) {
   const int per_split = m_tiles * n_tiles;
   ks = w / per_split;
@@ -256,20 +268,39 @@ __device__ __forceinline__ void epilogue32(const GemmParams& p, float gate_t, ui
 }
 
 // ----------------------------------------------------------------------------------------------
-// Shared memory: the TMA ring, then per consumer warpgroup a 64 x 64 fp32 accumulator slab (the register fragments
-// of half the tile's columns, re-read lane = row by the epilogue), then the per-warp epilogue staging tiles.
+// Shared memory: the TMA ring of 4 stages (a stage holds A, then B), then the per-warp epilogue staging tiles.
+// The epilogue moves accumulator fragments through 64 x 64 fp32 slabs (one per consumer warpgroup), re-read lane = row:
+//   narrow: one slab pair, in the ring space the 32 KiB stages leave free;
+//   wide  : the tile's last 4 ring stages, one per quarter of the columns (see the consumer).
 struct SmemLayout {
-  static constexpr int A_BYTES = BM * BK * 2;   // 16 KiB
-  static constexpr int B_BYTES = BN * BK * 2;   // 16 KiB
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int A_BYTES = BM * BK * 2;                        // 16 KiB
+  static constexpr int B_PART_BYTES = BN * BK * 2;                   // 16 KiB: the B rows one CTA loads
+  static constexpr int NARROW_STAGE_BYTES = A_BYTES + B_PART_BYTES;  // 32 KiB
+  static constexpr int WIDE_STAGE_BYTES = A_BYTES + CLUSTER * B_PART_BYTES;   // 48 KiB
+  static constexpr int STAGES = 4;
+  static constexpr int RING_BYTES = STAGES * WIDE_STAGE_BYTES;
   static constexpr int ACC_PITCH = 64 + 8;      // floats; 8 mod 32 keeps the fragment stores conflict-free
   static constexpr int ACC_BYTES = 64 * ACC_PITCH * 4;
-  static constexpr int ACC_OFF = STAGES * STAGE_BYTES;
-  static constexpr int EPI_OFF = ACC_OFF + NUM_CONSUMER_WG * ACC_BYTES;
+  static constexpr int ACC_OFF = STAGES * NARROW_STAGE_BYTES;   // narrow only
+  static_assert(ACC_OFF + NUM_CONSUMER_WG * ACC_BYTES <= RING_BYTES, "the narrow slabs fit beside the narrow ring");
+  static_assert(NUM_CONSUMER_WG * ACC_BYTES <= WIDE_STAGE_BYTES, "a parked quarter fits a wide stage");
+  static constexpr int EPI_OFF = RING_BYTES;
   static constexpr int BAR_OFF = EPI_OFF + NUM_EPI_WARPS * STAGE_BYTES_PER_WARP;
   static constexpr int TOTAL = BAR_OFF + 256 + 1024;   // + barriers + alignment slack
 };
 static_assert(SmemLayout::TOTAL <= 227 * 1024, "GEMM shared memory exceeds the sm_90 per-block limit");
+
+// Accumulator fragments of columns [64 h, 64 h + 64) -> a 64 x 64 fp32 slab (pitch ACC_PITCH), for lane = row re-reads.
+template <int NACC>
+__device__ __forceinline__ void park_part(float* slab, const float (&d)[NACC], int h, int wl, int lane) {
+  const int fr = 16 * wl + lane / 4, fc = 2 * (lane % 4);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int i = 4 * (8 * h + j);
+    *reinterpret_cast<float2*>(slab + fr * SmemLayout::ACC_PITCH + 8 * j + fc) = make_float2(d[i], d[i + 1]);
+    *reinterpret_cast<float2*>(slab + (fr + 8) * SmemLayout::ACC_PITCH + 8 * j + fc) = make_float2(d[i + 2], d[i + 3]);
+  }
+}
 
 template <int A_MN, int B_MN, int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
@@ -279,23 +310,41 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
-  uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* empty_bar = full_bar + L::STAGES;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
+  // Wide: the CTAs of a cluster walk the work items together (consecutive blockIdx.x form a cluster); CTA `crank`
+  // takes m-tile 2 * unit + crank and loads B rows [128 crank, 128 crank + 128) of the tile for both.  When the
+  // m-tile count is odd, the last pair's second tile lies wholly past M: it still loads (TMA fills zeros) and
+  // arrives, and its stores are masked by row < M.
+  const bool wide = p.wide != 0;
+  const int bn = wide ? BN_WIDE : BN;
+  const int stage_bytes = wide ? L::WIDE_STAGE_BYTES : L::NARROW_STAGE_BYTES;
+  const int crank = wide ? (int)cluster_ctarank() : 0;
+  const int walker = wide ? blockIdx.x / CLUSTER : blockIdx.x;
+  const int walkers = wide ? gridDim.x / CLUSTER : gridDim.x;
   const int m_tiles = (p.M + BM - 1) / BM;
-  const int n_tiles = (p.N + BN - 1) / BN;
-  const int num_work = m_tiles * n_tiles * p.splits;
+  const int m_units = wide ? (m_tiles + 1) / 2 : m_tiles;
+  const int n_tiles = (p.N + bn - 1) / bn;
+  const int num_work = m_units * n_tiles * p.splits;
   const int total_kb = (p.K + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], NUM_EPI_WARPS); }
+    // wide: a stage is freed only when the consumers of BOTH CTAs are done with it, since the partner's producer
+    // multicasts into this CTA's copy of the stage
+    for (int s = 0; s < L::STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], NUM_EPI_WARPS * (wide ? CLUSTER : 1));
+    }
     fence_barrier_init();
   }
-  __syncthreads();
+  // wide: the partner's barriers must be initialised before anything is multicast or arrived on them
+  if (wide) cluster_sync();
+  else __syncthreads();
 
   if (warp < 4) {
     // ===================== TMA producer (one thread) =====================
@@ -303,17 +352,17 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
     if (warp == 0 && lane == 0) {
       int stage = 0; uint32_t phase = 0;
-      for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-        int mt, nt, ks;
-        work_to_tile(w, m_tiles, n_tiles, mt, nt, ks);
-        const int m0 = mt * BM, n0 = nt * BN;
+      for (int w = walker; w < num_work; w += walkers) {
+        int mu, nt, ks;
+        work_to_tile(w, m_units, n_tiles, mu, nt, ks);
+        const int m0 = (wide ? 2 * mu + crank : mu) * BM, n0 = nt * bn;
         const int kb0 = ks * p.kb_per_split;
         const int kb1 = min(total_kb, kb0 + p.kb_per_split);
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * L::STAGE_BYTES;
+          uint8_t* sa = smem + stage * stage_bytes;
           uint8_t* sb = sa + L::A_BYTES;
-          mbar_arrive_expect_tx(&full_bar[stage], L::STAGE_BYTES);
+          mbar_arrive_expect_tx(&full_bar[stage], stage_bytes);
           const int k0 = kb * BK;
           if constexpr (A_MN == 0) {
             tma_load_2d(sa, &tma_a, &full_bar[stage], k0, m0);             // box {64 k, 128 rows}
@@ -322,14 +371,21 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
             for (int i = 0; i < BM / 64; ++i)                               // boxes {64 mn, 64 k}
               tma_load_2d(sa + i * (BK * 128), &tma_a, &full_bar[stage], m0 + 64 * i, (int)map_rows(k0, p.ak_rpg, p.ak_gs, p.ak_go));
           }
+          // this CTA's BN rows of B, at their place in the tile's B stage (the same in both layouts: K-major 8-row
+          // groups and MN-major 64-wide chunks are both BN * 128 B per BN rows)
+          uint8_t* sbp = sb + crank * L::B_PART_BYTES;
+          const int nb0 = n0 + crank * BN;
           if constexpr (B_MN == 0) {
-            tma_load_2d(sb, &tma_b, &full_bar[stage], k0, n0);             // box {64 k, 128 rows}
+            if (wide) tma_load_2d_multicast(sbp, &tma_b, &full_bar[stage], k0, nb0, (1u << CLUSTER) - 1);
+            else tma_load_2d(sbp, &tma_b, &full_bar[stage], k0, nb0);   // box {64 k, 128 rows}
           } else {
 #pragma unroll
-            for (int i = 0; i < BN / 64; ++i)
-              tma_load_2d(sb + i * (BK * 128), &tma_b, &full_bar[stage], n0 + 64 * i, k0);
+            for (int i = 0; i < BN / 64; ++i) {
+              if (wide) tma_load_2d_multicast(sbp + i * (BK * 128), &tma_b, &full_bar[stage], nb0 + 64 * i, k0, (1u << CLUSTER) - 1);
+              else tma_load_2d(sbp + i * (BK * 128), &tma_b, &full_bar[stage], nb0 + 64 * i, k0);
+            }
           }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          if (++stage == L::STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
@@ -347,77 +403,126 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
   if constexpr (EPI == OFK_EPI_GATE_RESID_F32) {
     if (p.gate != nullptr) gate_t = tanhf(__ldg(p.gate));
   }
-  int stage = 0; uint32_t phase = 0;
-  float d[64];
-  for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-    int mt, nt, ks;
-    work_to_tile(w, m_tiles, n_tiles, mt, nt, ks);
-    const int kb0 = ks * p.kb_per_split;
-    const int kb1 = min(total_kb, kb0 + p.kb_per_split);
-    int prev_stage = -1;
-    for (int kb = kb0; kb < kb1; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES);
-      const uint32_t sb = sa + L::A_BYTES;
-      wgmma_fence();
+  // one copy of the consumer loop per tile shape, so that the narrow one carries none of the wide one's state
+  auto consume = [&](auto wide_c) {
+    constexpr bool WIDE = decltype(wide_c)::value;
+    constexpr int TILE_N = WIDE ? BN_WIDE : BN;
+    constexpr int STAGE_BYTES = WIDE ? L::WIDE_STAGE_BYTES : L::NARROW_STAGE_BYTES;
+    auto release = [&](int s) {
+      if (lane != 0) return;
+      if constexpr (WIDE) {
 #pragma unroll
-      for (int k = 0; k < BK / WGMMA_K; ++k) {
+        for (int r = 0; r < CLUSTER; ++r) mbar_arrive_cluster(&empty_bar[s], r);
+      } else {
+        mbar_arrive(&empty_bar[s]);
+      }
+    };
+    int stage = 0; uint32_t phase = 0;
+    float d[TILE_N / 2];
+    for (int w = walker; w < num_work; w += walkers) {
+      int mu, nt, ks;
+      work_to_tile(w, m_units, n_tiles, mu, nt, ks);
+      const int mt = WIDE ? 2 * mu + crank : mu;
+      const int kb0 = ks * p.kb_per_split;
+      const int kb1 = min(total_kb, kb0 + p.kb_per_split);
+      // The first k-step overwrites the accumulators (scale-d = 0), but wgmma still names them as inputs: zeroing them
+      // here ends the previous tile's values at the epilogue instead of keeping all 128 live through it.
+#pragma unroll
+      for (int i = 0; i < TILE_N / 2; ++i) d[i] = 0.f;
+      int prev_stage = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+        const uint32_t sb = sa + L::A_BYTES;
         // K-major : this warpgroup's 64 rows start 64 * 128 B in; 8-row groups 1024 B apart (SBO); advance 32 B per
         //           WGMMA_K inside the swizzle atom.
         // MN-major: 64-wide MN chunks BK * 128 B apart (LBO; this warpgroup's rows are chunk `wg`), 8-k groups 1024 B
         //           apart (SBO); advance 2 k-groups = 2048 B per WGMMA_K.
-        const uint64_t adesc = A_MN ? make_wgmma_desc_sw128(sa + wg * (BK * 128) + k * 2048, BK * 128, 1024)
-                                    : make_wgmma_desc_sw128(sa + wg * (64 * 128) + k * 32, 16, 1024);
-        const uint64_t bdesc = B_MN ? make_wgmma_desc_sw128(sb + k * 2048, BK * 128, 1024)
-                                    : make_wgmma_desc_sw128(sb + k * 32, 16, 1024);
-        wgmma_m64n128k16_bf16<A_MN, B_MN>(d, adesc, bdesc, (kb > kb0 || k > 0) ? 1u : 0u);
-      }
-      wgmma_commit();
-      // keep one k-block of MMAs in flight; the one before it has retired, so its ring slot can be refilled
-      wgmma_wait<1>();
-      if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-      prev_stage = stage;
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
-    }
-    wgmma_wait<0>();
-    if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-
-    // Epilogue, in two halves of 64 columns: fragments -> slab, then each warp re-reads one 32 x 32 block with
-    // lane = row and runs the shared fused epilogue on it.
-    const int rh = wl & 1, ch = wl >> 1;
-    const int row0 = mt * BM + wg * 64 + rh * 32;
-    constexpr int AUXB = AuxBytes<EPI>::value;
+        auto adesc = [&](int k) {
+          return A_MN ? make_wgmma_desc_sw128(sa + wg * (BK * 128) + k * 2048, BK * 128, 1024)
+                      : make_wgmma_desc_sw128(sa + wg * (64 * 128) + k * 32, 16, 1024);
+        };
+        auto bdesc = [&](int k) {
+          return B_MN ? make_wgmma_desc_sw128(sb + k * 2048, BK * 128, 1024) : make_wgmma_desc_sw128(sb + k * 32, 16, 1024);
+        };
+        wgmma_fence();
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      named_bar_sync(1 + wg, 128);           // the previous half's readers are done with the slab
-      const int fr = 16 * wl + lane / 4, fc = 2 * (lane % 4);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int i = 4 * (8 * h + j);
-        *reinterpret_cast<float2*>(acc_slab + fr * L::ACC_PITCH + 8 * j + fc) = make_float2(d[i], d[i + 1]);
-        *reinterpret_cast<float2*>(acc_slab + (fr + 8) * L::ACC_PITCH + 8 * j + fc) = make_float2(d[i + 2], d[i + 3]);
-      }
-      named_bar_sync(1 + wg, 128);
-      uint32_t acc[32];
-      const float* src = acc_slab + (rh * 32 + lane) * L::ACC_PITCH + ch * 32;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float4 v = *reinterpret_cast<const float4*>(src + 4 * i);
-        acc[4 * i] = __float_as_uint(v.x); acc[4 * i + 1] = __float_as_uint(v.y);
-        acc[4 * i + 2] = __float_as_uint(v.z); acc[4 * i + 3] = __float_as_uint(v.w);
-      }
-      const int col = nt * BN + h * 64 + ch * 32;
-      if (row0 < p.M && col < p.N) {                                                 // warp-uniform
-        uint32_t aux_row[AUXB ? AUXB * 8 : 1];
-        if constexpr (AUXB != 0) {
-          uint4 pre[AUXB * 2];
-          aux_prefetch<AUXB>(pre, p.aux, p.ldaux, row0, col, p.M, p.N);
-          aux_commit<AUXB>(stage_addr, pre, aux_row);
+        for (int k = 0; k < BK / WGMMA_K; ++k) {
+          if constexpr (WIDE) wgmma_m64n256k16_bf16<A_MN, B_MN>(d, adesc(k), bdesc(k), (kb > kb0 || k > 0) ? 1u : 0u);
+          else wgmma_m64n128k16_bf16<A_MN, B_MN>(d, adesc(k), bdesc(k), (kb > kb0 || k > 0) ? 1u : 0u);
         }
-        epilogue32<EPI>(p, gate_t, stage_addr, row0, col, acc, aux_row);
+        wgmma_commit();
+        // keep one k-block of MMAs in flight; the one before it has retired, so its ring slot can be refilled
+        wgmma_wait<1>();
+        // wide: the stages of the tile's last STAGES k-blocks are kept for the epilogue
+        if (prev_stage >= 0 && !(WIDE && kb > kb1 - L::STAGES)) release(prev_stage);
+        prev_stage = stage;
+        if (++stage == L::STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+
+      // Epilogue, in parts of 64 columns: fragments -> a 64 x 64 slab, then each warp re-reads one 32 x 32 block with
+      // lane = row and runs the shared fused epilogue on it.
+      const int rh = wl & 1, ch = wl >> 1;
+      const int row0 = mt * BM + wg * 64 + rh * 32;
+      constexpr int AUXB = AuxBytes<EPI>::value;
+      auto run_part = [&](const float* slab, int col0) {
+        uint32_t acc[32];
+        const float* src = slab + (rh * 32 + lane) * L::ACC_PITCH + ch * 32;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float4 v = *reinterpret_cast<const float4*>(src + 4 * i);
+          acc[4 * i] = __float_as_uint(v.x); acc[4 * i + 1] = __float_as_uint(v.y);
+          acc[4 * i + 2] = __float_as_uint(v.z); acc[4 * i + 3] = __float_as_uint(v.w);
+        }
+        const int col = col0 + ch * 32;
+        if (row0 < p.M && col < p.N) {                                                 // warp-uniform
+          uint32_t aux_row[AUXB ? AUXB * 8 : 1];
+          if constexpr (AUXB != 0) {
+            uint4 pre[AUXB * 2];
+            aux_prefetch<AUXB>(pre, p.aux, p.ldaux, row0, col, p.M, p.N);
+            aux_commit<AUXB>(stage_addr, pre, aux_row);
+          }
+          epilogue32<EPI>(p, gate_t, stage_addr, row0, col, acc, aux_row);
+        }
+      };
+      if constexpr (!WIDE) {
+        release(prev_stage);
+#pragma unroll
+        for (int h = 0; h < BN / 64; ++h) {
+          named_bar_sync(1 + wg, 128);         // the previous part's readers are done with the slab
+          park_part(acc_slab, d, h, wl, lane);
+          named_bar_sync(1 + wg, 128);
+          run_part(acc_slab, nt * BN + h * 64);
+        }
+      } else {
+        // The kernel has 168 registers per thread; 128 live accumulators would leave the epilogue too few.  So all four
+        // quarters leave the registers first, into the ring stages of the tile's last four k-blocks (a wide tile has
+        // at least STAGES k-blocks), each returned to the producer once its quarter has been read.  Both warpgroups
+        // must be done with those stages' operands.
+        named_bar_sync(1 + NUM_CONSUMER_WG, 128 * NUM_CONSUMER_WG);
+        auto part_stage = [&](int h) { return (prev_stage + 1 + h) % L::STAGES; };   // h = 3: the last k-block's
+        auto part = [&](int h) { return reinterpret_cast<float*>(smem + part_stage(h) * STAGE_BYTES + wg * L::ACC_BYTES); };
+#pragma unroll
+        for (int h = 0; h < BN_WIDE / 64; ++h) park_part(part(h), d, h, wl, lane);
+        named_bar_sync(1 + wg, 128);
+#pragma unroll 1
+        for (int h = 0; h < BN_WIDE / 64; ++h) {
+          run_part(part(h), nt * BN_WIDE + h * 64);
+          // the TMA (async proxy) refill of the stage must not overtake these generic-proxy accesses
+          fence_proxy_async_smem();
+          __syncwarp();
+          release(part_stage(h));
+        }
       }
     }
-  }
+    // wide: neither CTA may exit while its partner can still arrive on its barriers (everything multicast into this
+    // CTA has been consumed by now).  The cluster barrier waits for non-exited threads only: the producer warpgroup
+    // has left.  (A barrier in the producer's code as well made ptxas hold the consumers to 168 registers, and spill.)
+    if constexpr (WIDE) cluster_sync();
+  };
+  if (wide) consume(std::true_type{});
+  else consume(std::false_type{});
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -495,21 +600,52 @@ static int get_tensor_map(const void* ptr, long long ld, int rows, int cols, int
 static int g_num_sms = 0;
 static int g_reserved_sms = 0;   // SMs the persistent grids leave free (ofk_gemm_reserve_sms): room for NCCL's CTAs
 
+// Persistent grid.  The wide shape is used when its work items fill every cluster slot at least once; below that,
+// 256-wide tiles would leave SMs idle (at M of a few rows, half of them on a weight-read-bound problem), and the
+// narrow shape runs.  Cluster slots come from the occupancy of this kernel's shared-memory size, since not every GPC
+// can hold an even number of these CTAs, less the reserved SMs, in whole clusters.
 template <int A_MN, int B_MN, int EPI>
-static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
+static int launch(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p, cudaStream_t stream) {
   auto kern = gemm_kernel<A_MN, B_MN, EPI>;
-  static bool attr_done = false;
-  if (!attr_done) {
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute cluster_attr;
+  cluster_attr.id = cudaLaunchAttributeClusterDimension;
+  cluster_attr.val.clusterDim.x = CLUSTER;
+  cluster_attr.val.clusterDim.y = 1;
+  cluster_attr.val.clusterDim.z = 1;
+  cfg.blockDim = dim3(NUM_THREADS);
+  cfg.dynamicSmemBytes = SmemLayout::TOTAL;
+  cfg.stream = stream;
+  static int max_clusters = -1;
+  if (max_clusters < 0) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemLayout::TOTAL);
     if (e != cudaSuccess) return ofk_set_error(OFK_ERR_CUDA, cudaGetErrorString(e));
-    attr_done = true;
+    cfg.gridDim = dim3(CLUSTER * g_num_sms);
+    cfg.attrs = &cluster_attr;
+    cfg.numAttrs = 1;
+    int n = 0;
+    e = cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
+    if (e != cudaSuccess) return ofk_set_error(OFK_ERR_CUDA, cudaGetErrorString(e));
+    max_clusters = n;
   }
-  const int m_tiles = (p.M + BM - 1) / BM, n_tiles = (p.N + BN - 1) / BN;
-  const int work = m_tiles * n_tiles * p.splits;
-  const int avail = g_num_sms - g_reserved_sms;
-  const int grid = work < avail ? work : avail;
-  kern<<<grid, NUM_THREADS, SmemLayout::TOTAL, stream>>>(ta, tb, p);
-  cudaError_t e = cudaGetLastError();
+  const int m_tiles = (p.M + BM - 1) / BM;
+  const int cluster_slots = (CLUSTER * max_clusters - g_reserved_sms) / CLUSTER;
+  const int wide_work = (m_tiles + 1) / 2 * ((p.N + BN_WIDE - 1) / BN_WIDE) * p.splits;
+  const int last_split_kb = (p.K + BK - 1) / BK - (p.splits - 1) * p.kb_per_split;   // the shortest split
+  p.wide = cluster_slots > 0 && wide_work >= cluster_slots && last_split_kb >= SmemLayout::STAGES;
+  if (p.wide) {
+    cfg.gridDim = dim3(CLUSTER * cluster_slots);
+    cfg.attrs = &cluster_attr;
+    cfg.numAttrs = 1;
+  } else {
+    const int work = m_tiles * ((p.N + BN - 1) / BN) * p.splits;
+    const int avail = g_num_sms - g_reserved_sms;
+    cfg.gridDim = dim3(work < avail ? work : avail);
+    cfg.attrs = nullptr;
+    cfg.numAttrs = 0;
+  }
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, p);
+  if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) return ofk_set_error(OFK_ERR_CUDA, cudaGetErrorString(e));
   ofk_count_launch();
   return 0;
@@ -597,6 +733,7 @@ static int gemm_impl(int epi, int a_mn_major, int b_mn_major, const void* A, lon
   p.splits = (total_kb + p.kb_per_split - 1) / p.kb_per_split;
   p.out = out; p.ldo = ldo; p.out2 = out2; p.ldo2 = ldo2; p.aux = aux; p.ldaux = ldaux; p.bias = bias; p.gate = gate;
   p.out_rpg = out_rpg; p.out_gs = out_gs; p.out_go = out_go; p.ak_rpg = ak_rpg; p.ak_gs = ak_gs; p.ak_go = ak_go;
+  p.wide = 0;   // chosen by launch()
   const int a_rows = ak_rpg > 0 ? (K / ak_rpg) * ak_gs : K;   // physical row count of an MN-major A
   {
     static int stream_mode = -1;   // OFK_GEMM_STREAM_OUT=0/1 overrides; default: stream when the outputs exceed ~32 MB
@@ -606,6 +743,7 @@ static int gemm_impl(int epi, int a_mn_major, int b_mn_major, const void* A, lon
   }
 
   // K-major: tensor [rows, K], box {64 (k), 128 rows}. MN-major: tensor [K, rows], box {64 (rows), 64 (k)}.
+  // A wide tile's B is two such 128-row boxes (K-major) or four 64-row ones, half of them loaded by each CTA.
   CUtensorMap ta, tb;
   int rc = a_mn_major ? get_tensor_map(A, lda, a_rows, M, 64, BK, &ta) : get_tensor_map(A, lda, M, K, BK, BM, &ta);
   if (rc) return rc;
