@@ -124,8 +124,13 @@ int ofk_layernorm_bwd(const void* dy, int dy_is_f32, long long lddy, int rows_pe
  *              1 = media mask, text_time == block+1  (torch.eq)       MaskedCrossAttention helpers.py:196-229
  *              2 = media mask, text_time >= block+1  (torch.ge)       only_attend_immediate_media=False
  *   text_time: [batch, nq] int32 (cumsum of media_locations, helpers.py:199-208); keys are grouped in
- *   blocks of `keys_per_media` (= 64 latents).  Rows with no allowed key (and, for mode 1, text_time == 0,
- *   helpers.py:223-229) produce exact zeros.
+ *   blocks of `keys_per_media` (the Perceiver's latent count: a multiple of 16 dividing nk).  Mode 1 rows with
+ *   text_time == 0 produce exact zeros (helpers.py:223-229) and LSE 0; any other row with no allowed key attends
+ *   uniformly over all nk keys and passes no gradient to q or k (masked_fill(-finfo.max) + softmax, helpers.py:218-221).
+ * Requirements (both directions): batch, heads, nq, nk >= 1 and batch, heads <= 65535 (OFK_ERR_ARG); q, k, v, o (and
+ *   d_o) 16-byte aligned with every batch and row stride a multiple of 8 elements; lse, delta and text_time 4-byte
+ *   aligned; dq, dk, dv 4-byte aligned with even batch and row strides (OFK_ERR_ALIGN).  Every argument is checked
+ *   before the first CUDA call.  Output rows are written whole; bytes outside them are never touched.
  */
 int ofk_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int batch, int heads, int nq,
                  int nk, long long q_bstride, long long ldq, long long k_bstride, long long ldk,
@@ -153,6 +158,12 @@ int ofk_attn_bwd(const void* q, const void* k, const void* v, const void* o, con
  *   diagonal -- a device-side decision, so no host synchronisation is needed to pick the fast path.
  *   lse: [batch, heads, nq] f32, log2 domain (consumed only by ofk_attn_dense_bwd).
  * Backward is dgrad only (the LM is frozen): dq/dk/dv bf16, fully overwritten.
+ * Requirements: head_dim 64 or 128; batch, heads, nq, nk >= 1 and batch, heads <= 65535; causal != 0 or a non-NULL
+ *   pure_causal_flag needs nq <= nk (OFK_ERR_ARG): the cache always holds the current chunk, and with nq > nk whole
+ *   query blocks would have no allowed key.  q, k, v, o (and d_o) 16-byte aligned with every batch and row stride a
+ *   multiple of 8 elements; lse, delta, slopes and pure_causal_flag 4-byte aligned; dq, dk, dv 4-byte aligned with
+ *   even batch and row strides (OFK_ERR_ALIGN).  mask is read byte by byte.  Every argument is checked before the
+ *   first CUDA call.
  */
 int ofk_attn_dense_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int batch, int heads,
                        int head_dim, int nq, int nk, long long q_bstride, long long ldq, long long k_bstride,

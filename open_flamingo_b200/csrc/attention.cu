@@ -629,7 +629,11 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const AttnPar
   }
 }
 
-static int check_common(const AttnParams& p) {
+static bool aligned(const void* ptr, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(ptr) & (bytes - 1)) == 0; }
+
+// q/k/v/o/dO are read (and o written) 16 bytes at a time per row and 32 bits at a time by the delta kernel; dq/dk/dv
+// are written 32 bits at a time; lse/delta/text_time are f32/int32 arrays.  Called before any CUDA call.
+static int check_common(const AttnParams& p, bool bwd) {
   if (p.batch <= 0 || p.heads <= 0 || p.nq <= 0 || p.nk <= 0) return ofk_set_error(OFK_ERR_ARG, "attention: empty problem");
   if (p.mask_mode < 0 || p.mask_mode > 2) return ofk_set_error(OFK_ERR_ARG, "attention: bad mask_mode");
   if (p.mask_mode != 0) {
@@ -637,8 +641,20 @@ static int check_common(const AttnParams& p) {
     if (p.kpm <= 0 || p.kpm % 16 != 0 || p.nk % p.kpm != 0)
       return ofk_set_error(OFK_ERR_ARG, "attention: keys_per_media must be a multiple of 16 dividing nk");
   }
-  if ((p.ldq | p.ldk | p.ldv | p.ldo) % 8 != 0) return ofk_set_error(OFK_ERR_ALIGN, "attention: row strides must be multiples of 8");
   if (p.batch > 65535 || p.heads > 65535) return ofk_set_error(OFK_ERR_ARG, "attention: batch/heads exceed grid limits");
+  const void* io = bwd ? static_cast<const void*>(p.o) : static_cast<const void*>(p.out);
+  if (!aligned(p.q, 16) || !aligned(p.k, 16) || !aligned(p.v, 16) || !aligned(io, 16) || (bwd && !aligned(p.d_o, 16)))
+    return ofk_set_error(OFK_ERR_ALIGN, "attention: q/k/v/o/dO must be 16-byte aligned");
+  if ((p.q_bs | p.ldq | p.k_bs | p.ldk | p.v_bs | p.ldv | p.o_bs | p.ldo) % 8 != 0)
+    return ofk_set_error(OFK_ERR_ALIGN, "attention: batch and row strides of q/k/v/o must be multiples of 8");
+  if (!aligned(p.lse, 4) || !aligned(p.delta, 4) || !aligned(p.text_time, 4))
+    return ofk_set_error(OFK_ERR_ALIGN, "attention: lse/delta/text_time must be 4-byte aligned");
+  if (bwd) {
+    if (!aligned(p.dq, 4) || !aligned(p.dk, 4) || !aligned(p.dv, 4))
+      return ofk_set_error(OFK_ERR_ALIGN, "attention bwd: dq/dk/dv must be 4-byte aligned");
+    if ((p.dq_bs | p.lddq | p.dk_bs | p.lddk | p.dv_bs | p.lddv) % 2 != 0)
+      return ofk_set_error(OFK_ERR_ALIGN, "attention bwd: grad strides must be even");
+  }
   return 0;
 }
 
@@ -656,7 +672,7 @@ extern "C" int ofk_attn_fwd(const void* q, const void* k, const void* v, void* o
   p.q_bs = q_bstride; p.ldq = ldq; p.k_bs = k_bstride; p.ldk = ldk; p.v_bs = v_bstride; p.ldv = ldv;
   p.o_bs = o_bstride; p.ldo = ldo; p.scale = scale; p.mask_mode = mask_mode; p.kpm = keys_per_media;
   if (!q || !k || !v || !o) return ofk_set_error(OFK_ERR_ARG, "attention: null pointer");
-  if (int rc = check_common(p)) return rc;
+  if (int rc = check_common(p, false)) return rc;
   dim3 grid((nq + BQ - 1) / BQ, heads, batch);
   if (ofk_attn_use_wgmma()) {
     attn_fwd_kernel<true><<<grid, ATT_THREADS, FWD_SMEM, (cudaStream_t)stream_>>>(p);
@@ -687,8 +703,7 @@ extern "C" int ofk_attn_bwd(const void* q, const void* k, const void* v, const v
   p.dv_bs = dv_bstride; p.lddv = lddv; p.scale = scale; p.mask_mode = mask_mode; p.kpm = keys_per_media;
   if (!q || !k || !v || !o || !d_o || !lse || !delta || !dq || !dk || !dv)
     return ofk_set_error(OFK_ERR_ARG, "attention bwd: null pointer");
-  if (int rc = check_common(p)) return rc;
-  if ((lddq | lddk | lddv) % 2 != 0) return ofk_set_error(OFK_ERR_ALIGN, "attention bwd: grad strides must be even");
+  if (int rc = check_common(p, true)) return rc;
   cudaStream_t stream = (cudaStream_t)stream_;
   const long long rows = (long long)batch * heads * nq;
   attn_delta_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(p);

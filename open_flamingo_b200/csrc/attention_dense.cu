@@ -560,11 +560,31 @@ __global__ void __launch_bounds__(THREADS) bwd_dkv_kernel(const Params p_in) {
   }
 }
 
-static int validate(const Params& p, int head_dim) {
+static bool aligned(const void* ptr, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(ptr) & (bytes - 1)) == 0; }
+
+// q/k/v/o/dO move 16 bytes at a time per row (32 bits in the delta kernel); dq/dk/dv are written 32 bits at a time;
+// lse, delta, slopes and the flag are 4-byte scalars.  The causal rule key <= row + nk - nq leaves whole query blocks
+// without a key when nq > nk, and the tile skipping would give those rows zeros instead of the finfo.min rule's uniform
+// attention; no caller needs that case, so it is rejected.  Called before any CUDA call.
+static int validate(const Params& p, int head_dim, bool bwd) {
   if (head_dim != 64 && head_dim != 128) return ofk_set_error(OFK_ERR_ARG, "dense attention: head_dim must be 64 or 128");
   if (p.batch <= 0 || p.heads <= 0 || p.nq <= 0 || p.nk <= 0) return ofk_set_error(OFK_ERR_ARG, "dense attention: empty problem");
-  if ((p.ldq | p.ldk | p.ldv | p.ldo) % 8 != 0) return ofk_set_error(OFK_ERR_ALIGN, "dense attention: row strides must be multiples of 8");
   if (p.batch > 65535 || p.heads > 65535) return ofk_set_error(OFK_ERR_ARG, "dense attention: batch/heads exceed grid limits");
+  if ((p.causal || p.pure_causal) && p.nq > p.nk)
+    return ofk_set_error(OFK_ERR_ARG, "dense attention: the causal rule needs nq <= nk");
+  const void* io = bwd ? static_cast<const void*>(p.o) : static_cast<const void*>(p.out);
+  if (!aligned(p.q, 16) || !aligned(p.k, 16) || !aligned(p.v, 16) || !aligned(io, 16) || (bwd && !aligned(p.d_o, 16)))
+    return ofk_set_error(OFK_ERR_ALIGN, "dense attention: q/k/v/o/dO must be 16-byte aligned");
+  if ((p.q_bs | p.ldq | p.k_bs | p.ldk | p.v_bs | p.ldv | p.o_bs | p.ldo) % 8 != 0)
+    return ofk_set_error(OFK_ERR_ALIGN, "dense attention: batch and row strides of q/k/v/o must be multiples of 8");
+  if (!aligned(p.lse, 4) || !aligned(p.delta, 4) || !aligned(p.slopes, 4) || !aligned(p.pure_causal, 4))
+    return ofk_set_error(OFK_ERR_ALIGN, "dense attention: lse/delta/slopes/pure_causal_flag must be 4-byte aligned");
+  if (bwd) {
+    if (!aligned(p.dq, 4) || !aligned(p.dk, 4) || !aligned(p.dv, 4))
+      return ofk_set_error(OFK_ERR_ALIGN, "dense attention bwd: dq/dk/dv must be 4-byte aligned");
+    if ((p.dq_bs | p.lddq | p.dk_bs | p.lddk | p.dv_bs | p.lddv) % 2 != 0)
+      return ofk_set_error(OFK_ERR_ALIGN, "dense attention bwd: grad strides must be even");
+  }
   return 0;
 }
 
@@ -629,7 +649,7 @@ extern "C" int ofk_attn_dense_fwd(const void* q, const void* k, const void* v, v
   p.q_bs = q_bstride; p.ldq = ldq; p.k_bs = k_bstride; p.ldk = ldk; p.v_bs = v_bstride; p.ldv = ldv; p.o_bs = o_bstride; p.ldo = ldo;
   p.scale = scale;
   if (!q || !k || !v || !o) return ofk_set_error(OFK_ERR_ARG, "dense attention: null pointer");
-  if (int rc = validate(p, head_dim)) return rc;
+  if (int rc = validate(p, head_dim, false)) return rc;
   return head_dim == 64 ? launch_fwd<64>(p, (cudaStream_t)stream) : launch_fwd<128>(p, (cudaStream_t)stream);
 }
 
@@ -649,6 +669,6 @@ extern "C" int ofk_attn_dense_bwd(const void* q, const void* k, const void* v, c
   p.q_bs = q_bstride; p.ldq = ldq; p.k_bs = k_bstride; p.ldk = ldk; p.v_bs = v_bstride; p.ldv = ldv; p.o_bs = o_bstride; p.ldo = ldo;
   p.dq_bs = dq_bstride; p.lddq = lddq; p.dk_bs = dk_bstride; p.lddk = lddk; p.dv_bs = dv_bstride; p.lddv = lddv; p.scale = scale;
   if (!q || !k || !v || !o || !d_o || !lse || !delta || !dq || !dk || !dv) return ofk_set_error(OFK_ERR_ARG, "dense attention bwd: null pointer");
-  if (int rc = validate(p, head_dim)) return rc;
+  if (int rc = validate(p, head_dim, true)) return rc;
   return head_dim == 64 ? launch_bwd<64>(p, (cudaStream_t)stream) : launch_bwd<128>(p, (cudaStream_t)stream);
 }

@@ -144,6 +144,45 @@ def _bstride_ld(t, name):
     return t.stride(0), t.stride(1)
 
 
+def _attn_qkv(q, k, v, inner):
+    """Shape checks shared by the attention wrappers; returns (B, nq, nk)."""
+    if q.dtype != bf16 or k.dtype != bf16 or v.dtype != bf16:
+        raise ValueError("attention operands must be bfloat16")
+    for t, name in ((q, "q"), (k, "k"), (v, "v")):
+        if t.dim() != 3 or t.shape[2] != inner:
+            raise ValueError(f"{name} must be [batch, rows, {inner}], got {tuple(t.shape)}")
+    if tuple(k.shape) != tuple(v.shape) or k.shape[0] != q.shape[0]:
+        raise ValueError(f"k {tuple(k.shape)} and v {tuple(v.shape)} must have the same shape and q's batch")
+    return q.shape[0], q.shape[1], k.shape[1]
+
+
+def _attn_rows(t, name, shape):
+    """An o / d_o / dq / dk / dv tensor: bf16 with exactly the given [batch, rows, heads*head_dim] shape."""
+    if t.dtype != bf16 or tuple(t.shape) != shape:
+        raise ValueError(f"{name} must be a bf16 tensor of shape {shape}, got {tuple(t.shape)} {t.dtype}")
+
+
+def _attn_lse(lse, B, heads, nq):
+    if lse.dtype != f32 or tuple(lse.shape) != (B, heads, nq) or not lse.is_contiguous():
+        raise ValueError(f"lse must be a contiguous float32 tensor of shape {(B, heads, nq)}")
+
+
+def _attn_text_time(text_time, B, nq):
+    if text_time is None or text_time.dtype != torch.int32 or tuple(text_time.shape) != (B, nq):
+        raise ValueError("media mask needs int32 text_time of shape [B, nq]")
+    return text_time.contiguous()
+
+
+def _dense_mask_slopes(mask, slopes, pure_causal_flag, B, heads, nq, nk):
+    # the kernel indexes mask as a contiguous [B, nq, nk] byte array and reads slopes[h]
+    if mask is not None and (tuple(mask.shape) != (B, nq, nk) or not mask.is_contiguous() or mask.element_size() != 1):
+        raise ValueError("mask must be a contiguous 1-byte tensor of shape [B, nq, nk]")
+    if slopes is not None and (slopes.dtype != f32 or slopes.numel() < heads or not slopes.is_contiguous()):
+        raise ValueError("slopes must be a contiguous float32 vector of length >= heads")
+    if pure_causal_flag is not None and (pure_causal_flag.dtype != torch.int32 or pure_causal_flag.numel() < 1):
+        raise ValueError("pure_causal_flag must be an int32 device tensor")
+
+
 def attn_force_legacy(on):
     """A/B switch: True = the mma.sync attention kernels, False = the wgmma kernels (the default).  Returns the
     previous setting."""
@@ -158,22 +197,18 @@ def attn_tc_launch_count():
 def attn_fwd(q, k, v, heads, scale, *, mask_mode=L.MASK_NONE, text_time=None, keys_per_media=64, out=None,
              want_lse=True):
     """q: [B, nq, heads*64] (may be a column-slice view), k/v: [B, nk, heads*64].  Returns (o, lse)."""
-    L.require_cuda(q, k, v)
-    B, nq = q.shape[0], q.shape[1]
-    nk = k.shape[1]
-    if q.dtype != bf16 or k.dtype != bf16 or v.dtype != bf16:
-        raise ValueError("attention operands must be bfloat16")
+    L.require_cuda(q, k, v, out, text_time)
+    B, nq, nk = _attn_qkv(q, k, v, heads * 64)
     if out is None:
         out = torch.empty((B, nq, heads * 64), device=q.device, dtype=bf16)
+    _attn_rows(out, "out", (B, nq, heads * 64))
     lse = torch.empty((B, heads, nq), device=q.device, dtype=f32) if want_lse else None
     qb, ldq = _bstride_ld(q, "q")
     kb, ldk = _bstride_ld(k, "k")
     vb, ldv = _bstride_ld(v, "v")
     ob, ldo = _bstride_ld(out, "out")
     if mask_mode != L.MASK_NONE:
-        if text_time is None or text_time.dtype != torch.int32 or tuple(text_time.shape) != (B, nq):
-            raise ValueError("media mask needs int32 text_time of shape [B, nq]")
-        text_time = text_time.contiguous()
+        text_time = _attn_text_time(text_time, B, nq)
     L.check(L.lib().ofk_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), L.ptr(lse), B, heads, nq, nk,
                                  qb, ldq, kb, ldk, vb, ldv, ob, ldo, scale, mask_mode, L.ptr(text_time), keys_per_media,
                                  L.stream_ptr()))
@@ -183,17 +218,25 @@ def attn_fwd(q, k, v, heads, scale, *, mask_mode=L.MASK_NONE, text_time=None, ke
 def attn_bwd(q, k, v, o, d_o, lse, heads, scale, *, mask_mode=L.MASK_NONE, text_time=None, keys_per_media=64,
              dq=None, dk=None, dv=None):
     """Returns (dq, dk, dv) bf16.  d_o must share o's strides."""
-    L.require_cuda(q, k, v, o, d_o)
-    B, nq = q.shape[0], q.shape[1]
-    nk = k.shape[1]
+    L.require_cuda(q, k, v, o, d_o, lse, dq, dk, dv, text_time)
+    inner = heads * 64
+    B, nq, nk = _attn_qkv(q, k, v, inner)
+    _attn_rows(o, "o", (B, nq, inner))
+    _attn_rows(d_o, "d_o", (B, nq, inner))
     if d_o.stride() != o.stride():
         raise ValueError("d_o must have the same strides as o")
+    _attn_lse(lse, B, heads, nq)
+    if mask_mode != L.MASK_NONE:
+        text_time = _attn_text_time(text_time, B, nq)
     if dq is None:
-        dq = torch.empty((B, nq, heads * 64), device=q.device, dtype=bf16)
+        dq = torch.empty((B, nq, inner), device=q.device, dtype=bf16)
     if dk is None:
-        dk = torch.empty((B, nk, heads * 64), device=q.device, dtype=bf16)
+        dk = torch.empty((B, nk, inner), device=q.device, dtype=bf16)
     if dv is None:
-        dv = torch.empty((B, nk, heads * 64), device=q.device, dtype=bf16)
+        dv = torch.empty((B, nk, inner), device=q.device, dtype=bf16)
+    _attn_rows(dq, "dq", (B, nq, inner))
+    _attn_rows(dk, "dk", (B, nk, inner))
+    _attn_rows(dv, "dv", (B, nk, inner))
     delta = torch.empty((B, heads, nq), device=q.device, dtype=f32)
     qb, ldq = _bstride_ld(q, "q")
     kb, ldk = _bstride_ld(k, "k")
@@ -202,8 +245,6 @@ def attn_bwd(q, k, v, o, d_o, lse, heads, scale, *, mask_mode=L.MASK_NONE, text_
     dqb, lddq = _bstride_ld(dq, "dq")
     dkb, lddk = _bstride_ld(dk, "dk")
     dvb, lddv = _bstride_ld(dv, "dv")
-    if text_time is not None:
-        text_time = text_time.contiguous()
     L.check(L.lib().ofk_attn_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), d_o.data_ptr(), lse.data_ptr(),
                                  delta.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, heads, nq, nk,
                                  qb, ldq, kb, ldk, vb, ldv, ob, ldo, dqb, lddq, dkb, lddk, dvb, lddv, scale, mask_mode,
@@ -327,16 +368,15 @@ def attn_dense_fwd(q, k, v, heads, head_dim, scale, *, causal=False, mask=None, 
                    want_lse=True):
     """Dense (LM self-attention) core: q/k/v [B, n, heads*head_dim] strided views; mask [B, nq, nk] bool/uint8
     (True = masked); slopes [heads] f32 ALiBi slopes.  Returns (o, lse)."""
-    L.require_cuda(q, k, v)
-    B, nq, nk = q.shape[0], q.shape[1], k.shape[1]
+    L.require_cuda(q, k, v, mask, slopes, pure_causal_flag)
+    B, nq, nk = _attn_qkv(q, k, v, heads * head_dim)
+    _dense_mask_slopes(mask, slopes, pure_causal_flag, B, heads, nq, nk)
     out = torch.empty((B, nq, heads * head_dim), device=q.device, dtype=bf16)
     lse = torch.empty((B, heads, nq), device=q.device, dtype=f32) if want_lse else None
     qb, ldq = _bstride_ld(q, "q")
     kb, ldk = _bstride_ld(k, "k")
     vb, ldv = _bstride_ld(v, "v")
     ob, ldo = _bstride_ld(out, "out")
-    if mask is not None and (tuple(mask.shape) != (B, nq, nk) or not mask.is_contiguous() or mask.element_size() != 1):
-        raise ValueError("mask must be a contiguous 1-byte tensor of shape [B, nq, nk]")
     L.check(L.lib().ofk_attn_dense_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), L.ptr(lse), B, heads,
                                        head_dim, nq, nk, qb, ldq, kb, ldk, vb, ldv, ob, ldo, scale, int(causal),
                                        L.ptr(mask), L.ptr(slopes), L.ptr(pure_causal_flag), L.stream_ptr()))
@@ -395,17 +435,24 @@ def attn_decode(q, k, v, heads, head_dim, scale, *, key_mask=None, slopes=None, 
 
 def attn_dense_bwd(q, k, v, o, d_o, lse, heads, head_dim, scale, *, causal=False, mask=None, slopes=None,
                    pure_causal_flag=None, dq=None, dk=None, dv=None):
-    L.require_cuda(q, k, v, o, d_o)
-    B, nq, nk = q.shape[0], q.shape[1], k.shape[1]
+    L.require_cuda(q, k, v, o, d_o, lse, mask, slopes, pure_causal_flag, dq, dk, dv)
+    inner = heads * head_dim
+    B, nq, nk = _attn_qkv(q, k, v, inner)
+    _attn_rows(o, "o", (B, nq, inner))
+    _attn_rows(d_o, "d_o", (B, nq, inner))
     if d_o.stride() != o.stride():
         raise ValueError("d_o must have the same strides as o")
-    inner = heads * head_dim
+    _attn_lse(lse, B, heads, nq)
+    _dense_mask_slopes(mask, slopes, pure_causal_flag, B, heads, nq, nk)
     if dq is None:
         dq = torch.empty((B, nq, inner), device=q.device, dtype=bf16)
     if dk is None:
         dk = torch.empty((B, nk, inner), device=q.device, dtype=bf16)
     if dv is None:
         dv = torch.empty((B, nk, inner), device=q.device, dtype=bf16)
+    _attn_rows(dq, "dq", (B, nq, inner))
+    _attn_rows(dk, "dk", (B, nk, inner))
+    _attn_rows(dv, "dv", (B, nk, inner))
     delta = torch.empty((B, heads, nq), device=q.device, dtype=f32)
     qb, ldq = _bstride_ld(q, "q")
     kb, ldk = _bstride_ld(k, "k")

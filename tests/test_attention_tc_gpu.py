@@ -25,16 +25,7 @@ def _media_run(ops, q, k, v, d_o, heads, scale, mode, tt, kpm):
     return o, lse, dq, dk, dv
 
 
-BIG = [
-    (32, 8, 256, 128, 1, 64),     # configs[1] gated cross-attention core
-    (8, 8, 512, 320, 1, 64),      # configs[3] (5 images): three key tiles -> bf16 red.add accumulation of dQ
-    (2, 8, 64, 4160, 0, 64),      # configs[4] Perceiver core (4096 visual tokens + 64 latents)
-    (2, 8, 192, 1088, 0, 64),     # many key tiles AND several query tiles: fp32 dQ accumulator + conversion pass
-    (4, 16, 257, 257, 0, 64),     # ViT-L/14
-]
-
-
-@pytest.mark.parametrize("case", CASES + BIG)
+@pytest.mark.parametrize("case", CASES)
 def test_media_attention_tc_vs_reference_and_legacy(ops, case):
     B, heads, nq, nk, mode, kpm = case
     torch.manual_seed(11)
@@ -105,8 +96,8 @@ def test_media_uniform_rows_tc(ops):
 
 
 def test_vit_tail_rows_split(ops):
-    """257 = 4 x 64 + 1 query rows (the ViT forward): the forward without an LSE gives the same output as the one
-    that also writes the LSE, and matches fp32 on the overhanging row."""
+    """257 = 4 x 64 + 1 query rows (the ViT forward): the forward without an LSE writes the same bits as the one that
+    also writes the LSE, overhanging row included, and matches fp32."""
     torch.manual_seed(19)
     B, heads, n = 3, 16, 257
     qkv = torch.randn(B, n, 3 * heads * 64, device="cuda").to(bf16)
@@ -118,8 +109,7 @@ def test_vit_tail_rows_split(ops):
     o_full, _ = ops.attn_fwd(q, k, v, heads, 0.125, want_lse=True)
     torch.cuda.synchronize()
     close(o_split, ref_attention(q, k, v, heads, 0.125, 0, None, 64), 2e-2, "vit split vs fp32")
-    assert torch.equal(o_split[:, :256], o_full[:, :256])
-    close(o_split[:, 256:], o_full[:, 256:], 1e-2, "tail row: without vs with LSE")
+    assert torch.equal(o_split, o_full)
 
 
 # ------------------------------------------------------------------ dense (LM self-attention) rules
