@@ -198,6 +198,32 @@ int ofk_attn_decode(const void* q, long long q_bstride, const void* k, const voi
                     float scale, const unsigned char* key_mask, long long mask_bstride, const float* slopes,
                     void* workspace, void* stream);
 
+/* The same decode attention with the key count in DEVICE memory, so that one captured CUDA graph serves every decode
+ * step: nk = min(*nk_dev, nk_max), read by the kernels.  The split plan is made on the device by the function the host
+ * uses for ofk_attn_decode, so the output at a given nk is bitwise identical to ofk_attn_decode at that nk, whatever
+ * nk_max is.  k/v, key_mask and slopes are as above with room for nk_max rows; no row at or past nk is read.
+ * *nk_dev <= 0 writes zeros.  workspace: >= ofk_attn_decode_workspace_bytes(batch, heads, head_dim, nk_max) bytes.
+ * Requirements: those of ofk_attn_decode with nk_max in place of nk, plus nk_dev non-NULL (OFK_ERR_ARG) and 4-byte
+ * aligned (OFK_ERR_ALIGN).  Every argument is checked before the first CUDA call. */
+int ofk_attn_decode_dev(const void* q, long long q_bstride, const void* k, const void* v, long long kv_bstride,
+                        long long ldkv, void* o, long long o_bstride, int batch, int heads, int head_dim, int nk_max,
+                        const int* nk_dev, float scale, const unsigned char* key_mask, long long mask_bstride,
+                        const float* slopes, void* workspace, void* stream);
+
+/* Append one K/V row per batch entry at a DEVICE-side position (the companion of ofk_attn_decode_dev in a captured
+ * decode step):  cache[b, *pos_dev, 0:width] = src[b, 0:width]  (bf16, 16-byte accesses), and, when key_mask is
+ * non-NULL, key_mask[b, *pos_dev] = (new_masked != NULL && new_masked[b] != 0)  (1 = the new token is padding).
+ *   src: [batch, width] rows (src_bstride); cache: [batch, capacity, >= width] (cache_bstride, row stride ld);
+ *   key_mask: [batch, >= capacity] bytes (mask_bstride) or NULL; new_masked: [batch] bytes or NULL (= unmasked).
+ * A position outside [0, capacity) writes nothing.
+ * Requirements: src, cache, pos_dev non-NULL; batch, width, capacity >= 1, batch <= 65535; ld >= width and
+ *   mask_bstride >= capacity (OFK_ERR_ARG); src and cache 16-byte aligned, pos_dev 4-byte aligned, width and every
+ *   stride of src and cache a multiple of 8 elements (OFK_ERR_ALIGN).  Every argument is checked before the first CUDA
+ *   call. */
+int ofk_kv_append(const void* src, long long src_bstride, void* cache, long long cache_bstride, long long ld,
+                  int batch, int width, int capacity, const int* pos_dev, unsigned char* key_mask,
+                  long long mask_bstride, const unsigned char* new_masked, void* stream);
+
 /* Attention implementation switch, for A/B measurements and for the parity tests that compare the two paths:
  * nonzero = the mma.sync kernels; 0 = the wgmma kernels (the default, unless the environment variable OFK_ATTN_LEGACY=1
  * is set when the library is loaded).  Returns the previous setting.

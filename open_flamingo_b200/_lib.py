@@ -65,6 +65,10 @@ _SIGNATURES = {
     "ofk_attn_decode_workspace_bytes": (c_ll, [c_int, c_int, c_int, c_int]),
     "ofk_attn_decode": (c_int, [c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_ll, c_void_p, c_ll, c_int, c_int, c_int,
                                 c_int, c_float, c_void_p, c_ll, c_void_p, c_void_p, c_void_p]),
+    "ofk_attn_decode_dev": (c_int, [c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_ll, c_void_p, c_ll, c_int, c_int, c_int,
+                                    c_int, c_void_p, c_float, c_void_p, c_ll, c_void_p, c_void_p, c_void_p]),
+    "ofk_kv_append": (c_int, [c_void_p, c_ll, c_void_p, c_ll, c_ll, c_int, c_int, c_int, c_void_p, c_void_p, c_ll,
+                              c_void_p, c_void_p]),
     "ofk_attn_force_legacy": (c_int, [c_int]),
     "ofk_attn_tc_launch_count": (c_ll, []),
     "ofk_text_time": (c_int, [c_void_p, c_ll, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),

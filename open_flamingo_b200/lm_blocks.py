@@ -93,6 +93,31 @@ def cached_block_forward(x, layer, mask, pure_flag, slopes, heads, eps, n1_w, wq
     return _block_tail(x2d, o.view(R, D), eps, wout, n2_w, wup, wdown)[0].view(B, nq, D)
 
 
+def decode_step_block_forward(x, layer, pos_nk, key_mask, new_masked, workspace, slopes, heads, eps, n1_w, wqkv, wout,
+                              n2_w, wup, wdown):
+    """cached_block_forward for one new token with its position on the device, so that the step can be captured in a
+    CUDA graph once and replayed at every position.  pos_nk: int32 [2] device tensor (cache row of the new token,
+    key count = row + 1); key_mask: the cache's [B, >= capacity] padding bytes; new_masked: uint8 [B], 1 where the new
+    token is padding; workspace: ops.decode_workspace at the layer's capacity.  The GEMMs have the shapes of the eager
+    path (q with N = D, K/V with N = 2D) and only the K/V destination differs -- a staging row that ops.kv_append
+    copies into the cache -- so the result is the eager path's, bit for bit.  x: [B, 1, D] f32; returns the same."""
+    B, _, D = x.shape
+    hd = D // heads
+    x2d = x.reshape(B, D)
+    if not x2d.is_contiguous():
+        x2d = x2d.contiguous()
+    xn, _, _ = ops.layernorm_fwd(x2d, n1_w, _zeros(D, x.device), eps, want_stats=False)
+    w = w16(wqkv)
+    q = ops.gemm(xn, w[:D])                                                         # [B, D]
+    kv = ops.gemm(xn, w[D:])                                                        # [B, 2D]
+    del xn
+    buf = layer.buf
+    ops.kv_append(kv, buf, pos_nk[0:1], key_mask=key_mask, new_masked=new_masked)
+    o = ops.attn_decode_dev(q, buf[..., :D], buf[..., D:], heads, hd, float(hd ** -0.5), pos_nk[1:2],
+                            key_mask=key_mask, slopes=slopes, workspace=workspace)
+    return _block_tail(x2d, o, eps, wout, n2_w, wup, wdown)[0].view(B, 1, D)
+
+
 class FrozenMptBlockFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, mask, pure_flag, slopes, heads, eps, n1_w, wqkv, wout, n2_w, wup, wdown):
@@ -187,6 +212,28 @@ class FastMptBlock:
             return False
         return True
 
+    def weights(self):
+        b = self.block
+        a = b.attn
+        return (b.norm_1.weight, a.Wqkv.weight, a.out_proj.weight, b.norm_2.weight, b.ffn.up_proj.weight,
+                b.ffn.down_proj.weight)
+
+    def slopes(self, device, position_bias=None):
+        """The block's ALiBi slopes on `device`, from `position_bias` or, if None, from the model's own builder."""
+        if self._slopes is None or self._slopes.device != device:
+            if position_bias is None:
+                from transformers.models.mpt.modeling_mpt import build_mpt_alibi_tensor
+                a = self.block.attn   # what MptModel.forward builds
+                position_bias = build_mpt_alibi_tensor(a.n_heads, a.max_seq_length, device=device)
+            self._slopes = _alibi_slopes(position_bias)
+        return self._slopes
+
+    def decode_step(self, x, layer, pos_nk, key_mask, new_masked, workspace):
+        """One captured decode step of this block (decode_step_block_forward)."""
+        a = self.block.attn
+        return decode_step_block_forward(x, layer, pos_nk, key_mask, new_masked, workspace, self.slopes(x.device),
+                                         a.n_heads, self.block.norm_1.eps, *self.weights())
+
     def applicable(self, hidden_states, position_bias, attention_mask, layer_past, use_cache, output_attentions):
         """The uncached path (FrozenMptBlockFn, forward and backward)."""
         if layer_past is not None or use_cache:
@@ -223,10 +270,8 @@ class FastMptBlock:
         b = self.block
         a = b.attn
         B, T, D = hidden_states.shape
-        if self._slopes is None or self._slopes.device != hidden_states.device:
-            self._slopes = _alibi_slopes(position_bias)
-            if self._slopes is None:
-                return None
+        if self.slopes(hidden_states.device, position_bias) is None:
+            return None
         nk = T if layer is None else layer.length + T
         decode = layer is not None and T == 1
         mask = None
@@ -246,8 +291,7 @@ class FastMptBlock:
                     mask = m.expand(B, 1, T, nk).reshape(B, T, nk).contiguous()
                 _mask_cache[0], _mask_cache[1], _mask_cache[2] = weakref.ref(m), mask, decode
         x = hidden_states if hidden_states.dtype == f32 else hidden_states.float()
-        weights = (b.norm_1.weight, a.Wqkv.weight, a.out_proj.weight, b.norm_2.weight, b.ffn.up_proj.weight,
-                   b.ffn.down_proj.weight)
+        weights = self.weights()
         flag = pure_causal_flag if mask is not None else None
         if layer is not None:
             out = cached_block_forward(x, layer, mask, flag, self._slopes, a.n_heads, b.norm_1.eps, *weights)

@@ -433,6 +433,83 @@ def attn_decode(q, k, v, heads, head_dim, scale, *, key_mask=None, slopes=None, 
     return out
 
 
+def decode_workspace(device, B, heads, head_dim, nk_max):
+    """A workspace of its own for attn_decode_dev: a captured graph keeps using the buffer it was captured with, so it
+    must not come from the grow-only per-stream buffers that eager calls may replace."""
+    need = int(L.lib().ofk_attn_decode_workspace_bytes(B, heads, head_dim, nk_max))
+    if need < 0:
+        raise ValueError(f"attn_decode: unsupported problem (batch {B}, heads {heads}, head_dim {head_dim}, "
+                         f"nk_max {nk_max})")
+    return torch.empty((need + 3) // 4, device=device, dtype=f32)
+
+
+def attn_decode_dev(q, k, v, heads, head_dim, scale, nk_dev, *, key_mask=None, slopes=None, out=None, workspace=None):
+    """attn_decode with the key count read on the device: nk = min(nk_dev[0], nk_max), nk_max = k.shape[1] (the cache's
+    capacity).  Bitwise equal to attn_decode over the first nk rows.  nk_dev: int32 CUDA tensor; workspace: a float32
+    tensor of at least ofk_attn_decode_workspace_bytes(B, heads, head_dim, nk_max) bytes (see decode_workspace)."""
+    L.require_cuda(q, k, v, key_mask, slopes, nk_dev, workspace)
+    if q.dtype != bf16 or k.dtype != bf16 or v.dtype != bf16:
+        raise ValueError("attention operands must be bfloat16")
+    inner = heads * head_dim
+    if q.dim() != 2 or q.shape[1] != inner or q.stride(1) != 1:
+        raise ValueError(f"q must be [B, {inner}] with unit inner stride, got {tuple(q.shape)} stride {q.stride()}")
+    B = q.shape[0]
+    if k.dim() != 3 or tuple(k.shape) != tuple(v.shape) or k.shape[0] != B or k.shape[2] != inner or \
+            k.stride(2) != 1 or k.stride() != v.stride():
+        raise ValueError(f"k/v must be [B, nk_max, {inner}] views with equal strides and unit inner stride, got "
+                         f"{tuple(k.shape)} {k.stride()} / {tuple(v.shape)} {v.stride()}")
+    nk_max = k.shape[1]
+    if key_mask is not None and (key_mask.dim() != 2 or key_mask.shape[0] != B or key_mask.shape[1] < nk_max or
+                                 key_mask.element_size() != 1 or key_mask.stride(1) != 1):
+        raise ValueError(f"key_mask must be a 1-byte [B, >= {nk_max}] tensor with unit inner stride")
+    if slopes is not None and (slopes.dtype != f32 or slopes.numel() < heads or not slopes.is_contiguous()):
+        raise ValueError("slopes must be a contiguous float32 vector of length >= heads")
+    if nk_dev.dtype != torch.int32 or nk_dev.numel() < 1:
+        raise ValueError("nk_dev must be an int32 device tensor")
+    if out is None:
+        out = torch.empty((B, inner), device=q.device, dtype=bf16)
+    elif out.dtype != bf16 or out.dim() != 2 or tuple(out.shape) != (B, inner) or out.stride(1) != 1:
+        raise ValueError(f"out must be a bf16 [B, {inner}] tensor with unit inner stride")
+    if workspace is None:
+        workspace = decode_workspace(q.device, B, heads, head_dim, nk_max)
+    elif workspace.numel() * workspace.element_size() < int(L.lib().ofk_attn_decode_workspace_bytes(
+            B, heads, head_dim, nk_max)):
+        raise ValueError("attn_decode_dev: workspace too small for nk_max")
+    L.check(L.lib().ofk_attn_decode_dev(q.data_ptr(), q.stride(0), k.data_ptr(), v.data_ptr(), k.stride(0), k.stride(1),
+                                        out.data_ptr(), out.stride(0), B, heads, head_dim, nk_max, nk_dev.data_ptr(),
+                                        scale, L.ptr(key_mask), 0 if key_mask is None else key_mask.stride(0),
+                                        L.ptr(slopes), workspace.data_ptr(), L.stream_ptr()))
+    return out
+
+
+def kv_append(src, cache, pos_dev, *, key_mask=None, new_masked=None):
+    """cache[b, pos, :] = src[b, :] at the device-side position pos = pos_dev[0] (nothing outside [0, capacity)), and
+    key_mask[b, pos] = new_masked[b] != 0 (0 when new_masked is None).  src: [B, W] bf16 with unit inner stride;
+    cache: [B, capacity, W] bf16 view with unit inner stride; key_mask: 1-byte [B, >= capacity] with unit inner stride;
+    new_masked: 1-byte [B]; pos_dev: int32 CUDA tensor."""
+    L.require_cuda(src, cache, pos_dev, key_mask, new_masked)
+    if src.dtype != bf16 or cache.dtype != bf16:
+        raise ValueError("kv_append operands must be bfloat16")
+    if src.dim() != 2 or src.stride(1) != 1:
+        raise ValueError(f"src must be [B, W] with unit inner stride, got {tuple(src.shape)} stride {src.stride()}")
+    B, W = src.shape
+    if cache.dim() != 3 or cache.shape[0] != B or cache.shape[2] != W or cache.stride(2) != 1:
+        raise ValueError(f"cache must be a [{B}, capacity, {W}] view with unit inner stride, got {tuple(cache.shape)}")
+    cap = cache.shape[1]
+    if key_mask is not None and (key_mask.dim() != 2 or key_mask.shape[0] != B or key_mask.shape[1] < cap or
+                                 key_mask.element_size() != 1 or key_mask.stride(1) != 1):
+        raise ValueError(f"key_mask must be a 1-byte [B, >= {cap}] tensor with unit inner stride")
+    if new_masked is not None and (new_masked.numel() != B or new_masked.element_size() != 1 or
+                                   not new_masked.is_contiguous()):
+        raise ValueError(f"new_masked must be a contiguous 1-byte tensor of {B} elements")
+    if pos_dev.dtype != torch.int32 or pos_dev.numel() < 1:
+        raise ValueError("pos_dev must be an int32 device tensor")
+    L.check(L.lib().ofk_kv_append(src.data_ptr(), src.stride(0), cache.data_ptr(), cache.stride(0), cache.stride(1), B,
+                                  W, cap, pos_dev.data_ptr(), L.ptr(key_mask),
+                                  0 if key_mask is None else key_mask.stride(0), L.ptr(new_masked), L.stream_ptr()))
+    return cache
+
+
 def attn_dense_bwd(q, k, v, o, d_o, lse, heads, head_dim, scale, *, causal=False, mask=None, slopes=None,
                    pure_causal_flag=None, dq=None, dk=None, dv=None):
     L.require_cuda(q, k, v, o, d_o, lse, mask, slopes, pure_causal_flag, dq, dk, dv)

@@ -10,6 +10,7 @@ data-parallel path replicates the model (OF-3B training fits one 80 GB H100) and
 import torch
 from torch import nn
 
+from .. import decode_graph
 from .helpers import PerceiverResampler
 
 
@@ -79,7 +80,9 @@ class Flamingo(nn.Module):
         """HF generate() conditioned on images; kwargs are forwarded (max_new_tokens, num_beams, ...).
         Returns lang_x with the generated tokens appended.  When generation uses a cache (`use_cache=True`) under
         bf16 autocast, the frozen MPT blocks decode on the kernels through a kv_cache.KVCache (see
-        FlamingoLMMixin.make_kv_cache)."""
+        FlamingoLMMixin.make_kv_cache).  `cache_implementation="static"` (HF's name for a fixed-capacity cache)
+        makes that cache fixed-capacity -- prompt plus new tokens, for every beam -- and replays one captured CUDA graph
+        per generated token (decode_graph); where the kernels' cache is not made, the argument goes to HF."""
         num_beams = kwargs.pop("num_beams", 1)
         if num_beams > 1:
             vision_x = vision_x.repeat_interleave(num_beams, dim=0)
@@ -89,7 +92,18 @@ class Flamingo(nn.Module):
             self._encode_vision_x(vision_x=vision_x)
             eos_token_id = kwargs.pop("eos_token_id", self.eoc_token_id)
             if kwargs.get("past_key_values") is None and kwargs.get("use_cache", lm.generation_config.use_cache):
-                cache = lm.make_kv_cache()   # bf16 decoding on the kernels; None keeps HF's DynamicCache
+                cache = None
+                if kwargs.get("cache_implementation") == "static":
+                    # HF's precedence: keyword arguments over the call's generation_config over the model's
+                    gc = kwargs.get("generation_config") or lm.generation_config
+                    capacity = decode_graph.static_cache_capacity(
+                        lang_x.shape[1], kwargs.get("max_new_tokens", gc.max_new_tokens),
+                        kwargs.get("max_length", gc.max_length))
+                    cache = lm.make_kv_cache(capacity=capacity)
+                    if cache is not None:
+                        kwargs.pop("cache_implementation")
+                if cache is None:
+                    cache = lm.make_kv_cache()   # bf16 decoding on the kernels; None keeps HF's DynamicCache
                 if cache is not None:
                     kwargs["past_key_values"] = cache
             output = lm.generate(input_ids=lang_x, attention_mask=attention_mask, eos_token_id=eos_token_id,

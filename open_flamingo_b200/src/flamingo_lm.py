@@ -11,7 +11,7 @@ PyTorch modules.
 import torch
 import torch.nn as nn
 
-from .. import lm_blocks
+from .. import decode_graph, lm_blocks
 from ..kv_cache import KVCache
 from .helpers import GatedCrossAttentionBlock
 from .utils import getattr_recursive, setattr_recursive
@@ -121,10 +121,26 @@ class FlamingoLMMixin(nn.Module):
             cache = self.make_kv_cache()   # a cached prefix (rank classification): decode its continuation on the kernels
             if cache is not None:
                 kwargs["past_key_values"] = cache
+        cache = kwargs.get("past_key_values")
+        fixed = isinstance(cache, KVCache) and cache.capacity is not None
+        if fixed:
+            cache.check_room(input_ids.shape[1])   # before any work is queued
         media_locations = input_ids == self.media_token_id
         # HF generate() feeds one token at a time after the prompt; such calls carry no <image> token and must
         # keep attending to the last cached image (flamingo_lm.py:137-146).
         use_cached = bool(self._use_cached_vision_x and self.is_conditioned() and not media_locations.any())
+        for layer in self._get_decoder_layers():
+            if not use_cached:
+                layer.condition_media_locations(media_locations)
+            layer.condition_use_cached_media(use_cached)
+        if fixed:
+            # a fixed-capacity cache: one-token steps replay a captured CUDA graph (decode_graph); any other step runs
+            # eagerly on the same buffers
+            if decode_graph.eligible(self, input_ids, attention_mask, cache, use_cached, kwargs):
+                out = self.decode_graphs.step(self, input_ids, attention_mask, cache)
+                if out is not None:
+                    return out
+            cache.note_key_padding(attention_mask, input_ids.shape[0], input_ids.shape[1], input_ids.device)
         # device-side "attention_mask is all ones" flag: lets the LM attention kernel take its pure-causal fast path
         # without a host synchronisation
         if input_ids.is_cuda:
@@ -133,9 +149,6 @@ class FlamingoLMMixin(nn.Module):
         else:
             flag = None
         for layer in self._get_decoder_layers():
-            if not use_cached:
-                layer.condition_media_locations(media_locations)
-            layer.condition_use_cached_media(use_cached)
             layer._pure_causal_flag = flag
         if input_ids.is_cuda and torch.cuda.is_current_stream_capturing() and type(self).__mro__[2].__name__.startswith("Mpt") \
                 and (attention_mask is None or attention_mask.dim() == 2) and kwargs.get("past_key_values") is None:
@@ -150,11 +163,16 @@ class FlamingoLMMixin(nn.Module):
             attention_mask = m4.contiguous()
         return super().forward(input_ids=input_ids, attention_mask=attention_mask, **kwargs)
 
-    def make_kv_cache(self):
+    def make_kv_cache(self, capacity=None):
         """A kv_cache.KVCache for decoding this LM on the kernels, or None where HF's own cache is kept: it is made only
         on CUDA, under `torch.autocast("cuda", dtype=torch.bfloat16)` (the caller asked for bf16 numerics; the cache
         stores bf16), with lm_blocks.ENABLED, and when every decoder block is a recognised MPT block.  In fp32 every
-        path stays HF's."""
+        path stays HF's.
+
+        capacity: None for a cache that grows; an int for a fixed-capacity cache of at least that many rows, with which
+        `forward(..., past_key_values=cache)` replays one captured CUDA graph per one-token step (decode_graph).  Its
+        buffers are allocated at the first write; each captured shape also keeps a cache's worth of rows until
+        `self.decode_graphs.clear()`."""
         if not lm_blocks.ENABLED or not torch.is_autocast_enabled("cuda") or \
                 torch.get_autocast_dtype("cuda") != torch.bfloat16:
             return None
@@ -163,7 +181,12 @@ class FlamingoLMMixin(nn.Module):
             return None
         if not self.get_input_embeddings().weight.is_cuda:
             return None
-        return KVCache(len(layers))
+        return KVCache(len(layers), capacity=capacity)
+
+    @property
+    def decode_graphs(self):
+        """The captured decode steps of this model (decode_graph.DecodeGraphs), made on first use."""
+        return decode_graph.graphs_for(self)
 
     def is_conditioned(self) -> bool:
         """All layers hold vis_x and media_locations (flamingo_lm.py:157-159)."""
