@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define OFK_ABI_VERSION 3
+#define OFK_ABI_VERSION 4
 
 enum {
   OFK_OK = 0,
@@ -115,9 +115,8 @@ int ofk_layernorm_bwd(const void* dy, int dy_is_f32, long long lddy, int rows_pe
 
 /* ------------------------------------------------------------------------------------------------
  * Attention core  O = softmax(scale * Q K^T + mask) V  per (batch, head), head_dim = 64, bf16 in/out,
- * fp32 softmax, online (flash-style).  Default: warpgroup kernels whose QK^T / PV (and the backward's five products) are
- * wgmma on 128-byte-swizzled shared-memory tiles, P / dS fed from registers; the mma.sync kernels of the same files are
- * the A/B reference (ofk_attn_force_legacy).
+ * fp32 softmax, online (flash-style).  Warpgroup kernels whose QK^T / PV (and the backward's five products) are wgmma on
+ * 128-byte-swizzled shared-memory tiles, P / dS fed from registers.
  *   q: [batch, nq, heads*64] (ldq row stride), k/v: [batch, nk, heads*64] (ldk/ldv), o like q (ldo).
  *   q_bstride/k_bstride...: batch strides in elements.  lse: [batch, heads, nq] f32 (log2 domain, for bwd).
  *   mask_mode: 0 = none                                              PerceiverAttention helpers.py:58-63, ViT MHA
@@ -148,8 +147,8 @@ int ofk_attn_bwd(const void* q, const void* k, const void* v, const void* o, con
 
 /* ------------------------------------------------------------------------------------------------
  * Dense self-attention core of the frozen LM's decoder blocks (HF MptAttention; reached via
- * flamingo_lm.py:63-65 -- SURVEY.md section 8f rank 1).  head_dim 64 or 128.  Same wgmma / mma.sync pair as above
- * (csrc/attention_dense.cu).
+ * flamingo_lm.py:63-65 -- SURVEY.md section 8f rank 1).  head_dim 64 or 128.  Same wgmma warpgroup kernels as above,
+ * on the same tile layer (csrc/attention_dense.cu, csrc/attention_tile.cuh).
  *   S = scale * Q K^T + slopes[h] * key_index  (ALiBi; slopes NULL = no bias)
  *   masked (mask[b, q, k] != 0, mask: [batch, nq, nk] bytes or NULL; and/or causal: key > query + nk - nq)
  *   scores take "finfo.min" exactly like masked_fill: a fully masked row attends uniformly.
@@ -223,13 +222,6 @@ int ofk_attn_decode_dev(const void* q, long long q_bstride, const void* k, const
 int ofk_kv_append(const void* src, long long src_bstride, void* cache, long long cache_bstride, long long ld,
                   int batch, int width, int capacity, const int* pos_dev, unsigned char* key_mask,
                   long long mask_bstride, const unsigned char* new_masked, void* stream);
-
-/* Attention implementation switch, for A/B measurements and for the parity tests that compare the two paths:
- * nonzero = the mma.sync kernels; 0 = the wgmma kernels (the default, unless the environment variable OFK_ATTN_LEGACY=1
- * is set when the library is loaded).  Returns the previous setting.
- * ofk_attn_tc_launch_count(): how many attention calls (forward or backward) the wgmma kernels have served. */
-int ofk_attn_force_legacy(int on);
-long long ofk_attn_tc_launch_count(void);
 
 /* ------------------------------------------------------------------------------------------------
  * Small fused elementwise / reduction kernels.

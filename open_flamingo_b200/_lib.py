@@ -69,8 +69,6 @@ _SIGNATURES = {
                                     c_int, c_void_p, c_float, c_void_p, c_ll, c_void_p, c_void_p, c_void_p]),
     "ofk_kv_append": (c_int, [c_void_p, c_ll, c_void_p, c_ll, c_ll, c_int, c_int, c_int, c_void_p, c_void_p, c_ll,
                               c_void_p, c_void_p]),
-    "ofk_attn_force_legacy": (c_int, [c_int]),
-    "ofk_attn_tc_launch_count": (c_ll, []),
     "ofk_text_time": (c_int, [c_void_p, c_ll, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "ofk_cast_f32_bf16": (c_int, [c_void_p, c_void_p, c_ll, c_void_p]),
     "ofk_reduce_workspace_bytes": (c_ll, []),
@@ -108,7 +106,7 @@ def lib():
             fn = getattr(L, name)  # AttributeError if the symbol is not exported
             fn.restype = res
             fn.argtypes = args
-        if L.ofk_abi_version() != 3:
+        if L.ofk_abi_version() != 4:
             raise RuntimeError("libofk.so ABI version mismatch")
         _lib = L
     return _lib

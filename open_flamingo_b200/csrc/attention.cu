@@ -19,16 +19,12 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "attention_tile.cuh"
 #include "ofk_internal.h"
-#include "ofk_ptx.cuh"
 
 namespace ofk {
 
 constexpr int HD = 64;    // head dim
-constexpr int BQ = 64;    // query rows per CTA (16 per warp)
-constexpr int BKV = 64;   // keys per tile
-constexpr int ATT_THREADS = 128;
-constexpr float LOG2E = 1.4426950408889634f;
 
 struct AttnParams {
   const __nv_bfloat16 *q, *k, *v, *o, *d_o;
@@ -42,144 +38,6 @@ struct AttnParams {
   float scale;
   int mask_mode, kpm;
 };
-
-// ---------------------------------------------------------------- smem tile helpers (64 rows x 64 bf16, swizzled)
-// The XOR pattern is the 128-byte swizzle wgmma descriptors expect; tiles start on 1024-byte boundaries.
-__device__ __forceinline__ uint32_t tile_off(int row, int chunk) {  // chunk = 16-byte column group 0..7
-  return (uint32_t)(row * 128 + ((chunk ^ (row & 7)) << 4));
-}
-
-__device__ __forceinline__ void cp_async16(uint32_t saddr, const void* g, bool valid) {
-  const int sz = valid ? 16 : 0;
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(saddr), "l"(g), "r"(sz) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-// Load rows [row0, row0+64) x 64 columns (starting at `g`, row stride ld) into a swizzled tile; rows >= nrows -> 0.
-__device__ __forceinline__ void load_tile(uint8_t* tile, const __nv_bfloat16* g, long long ld, int row0, int nrows) {
-  const uint32_t base = smem_u32(tile);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int idx = threadIdx.x + i * ATT_THREADS;  // 0..511
-    const int r = idx >> 3, c = idx & 7;
-    const bool valid = (row0 + r) < nrows;
-    const __nv_bfloat16* src = g + (long long)(valid ? (row0 + r) : 0) * ld + c * 8;
-    cp_async16(base + tile_off(r, c), src, valid);
-  }
-}
-
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-// A fragments (16 rows x 64 k) of a row-major tile: rows [r0, r0+16).
-__device__ __forceinline__ void load_a_frags(const uint8_t* tile, int r0, uint32_t (&a)[4][4]) {
-  const int lane = threadIdx.x & 31;
-  const int row = r0 + (lane & 7) + ((lane >> 3) & 1) * 8;
-  const uint32_t base = smem_u32(tile);
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks) {
-    const int chunk = ks * 2 + (lane >> 4);
-    ldsm_x4(base + tile_off(row, chunk), a[ks][0], a[ks][1], a[ks][2], a[ks][3]);
-  }
-}
-
-// Tensor-core products of one CTA = one warpgroup of 4 warps x 16 rows.  WG = true: one warpgroup-wide wgmma per 16-deep
-// k step over all 64 rows (A from each warp's registers, B from the 128-byte-swizzled tile through a descriptor);
-// WG = false: per-warp mma.sync, kept as the A/B reference.  Both use the same accumulator and A-fragment layout, so
-// the softmax / mask code around them is shared.
-__device__ __forceinline__ void wgmma_pin(float* d, int n) {
-  for (int i = 0; i < n; ++i) asm volatile("" : "+f"(d[i])::"memory");
-}
-
-// C[16 x 64] (+)= A[16 x 64(k)] * T^T where T is a [64 n][64 k] row-major tile  ("n rows, k contiguous").  A is the
-// warp's rows of `atile` (WG: read by wgmma through a descriptor of the whole 64-row tile) or, for mma.sync, the
-// fragments `a` already loaded from it.
-template <bool WG>
-__device__ __forceinline__ void mma_a_tileT(float (&c)[8][4], const uint32_t (&a)[4][4], const uint8_t* atile,
-                                            const uint8_t* tile) {
-  const uint32_t base = smem_u32(tile);
-  if constexpr (WG) {
-    const uint32_t abase = smem_u32(atile);
-    float(&d)[32] = *reinterpret_cast<float(*)[32]>(&c[0][0]);
-    wgmma_pin(d, 32);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks)
-      wgmma_m64n64k16_ss(d, make_wgmma_desc_sw128(abase + ks * 32, 16, 1024), make_wgmma_desc_sw128(base + ks * 32, 16, 1024));
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_pin(d, 32);
-  } else {
-    const int lane = threadIdx.x & 31;
-#pragma unroll
-    for (int np = 0; np < 4; ++np) {       // pairs of 8-wide n tiles
-      const int nrow = np * 16 + (lane & 7) + (lane >> 4) * 8;
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        uint32_t b0, b1, b2, b3;
-        const int chunk = ks * 2 + ((lane >> 3) & 1);
-        ldsm_x4(base + tile_off(nrow, chunk), b0, b1, b2, b3);
-        mma16816(c[np * 2], a[ks], b0, b1);
-        mma16816(c[np * 2 + 1], a[ks], b2, b3);
-      }
-    }
-  }
-}
-
-// C[16 x 64(n)] += P[16 x 64(k)] * T where T is a [64 k][64 n] row-major tile ("k rows, n contiguous").
-template <bool WG>
-__device__ __forceinline__ void mma_p_tile(float (&c)[8][4], const uint32_t (&p)[4][4], const uint8_t* tile) {
-  const uint32_t base = smem_u32(tile);
-  if constexpr (WG) {
-    float(&d)[32] = *reinterpret_cast<float(*)[32]>(&c[0][0]);
-    wgmma_pin(d, 32);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) wgmma_m64n64k16_rs<1>(d, p[ks], make_wgmma_desc_sw128(base + ks * 2048, 8192, 1024));
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_pin(d, 32);
-  } else {
-    const int lane = threadIdx.x & 31;
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      const int krow = ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
-#pragma unroll
-      for (int np = 0; np < 4; ++np) {
-        uint32_t b0, b1, b2, b3;
-        const int chunk = np * 2 + (lane >> 4);
-        ldsm_x4_t(base + tile_off(krow, chunk), b0, b1, b2, b3);
-        mma16816(c[np * 2], p[ks], b0, b1);
-        mma16816(c[np * 2 + 1], p[ks], b2, b3);
-      }
-    }
-  }
-}
-
-// Pack a C-layout [16 x 64] fp32 tile into A-layout bf16 fragments (k = the 64 columns).
-__device__ __forceinline__ void c_to_a(const float (&c)[8][4], uint32_t (&a)[4][4]) {
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks) {
-    a[ks][0] = pack_bf16x2(c[2 * ks][0], c[2 * ks][1]);
-    a[ks][1] = pack_bf16x2(c[2 * ks][2], c[2 * ks][3]);
-    a[ks][2] = pack_bf16x2(c[2 * ks + 1][0], c[2 * ks + 1][1]);
-    a[ks][3] = pack_bf16x2(c[2 * ks + 1][2], c[2 * ks + 1][3]);
-  }
-}
 
 // Row classification for the media mask.
 //   kind 0: normal masked row; 1: zero row; 2: uniform row (all keys, S = 0, no grad to q/k); 3: unmasked
@@ -243,16 +101,12 @@ __device__ __forceinline__ void block_key_range(const AttnParams& p, int b, int 
 }
 
 // ================================================================ forward
-// Tiles live in dynamic shared memory aligned by hand: the 128-byte swizzle wgmma reads is a function of the absolute
-// shared address, so every tile must start on a 1024-byte boundary.
-constexpr int FWD_SMEM = 5 * 64 * 128 + 1024;
-extern __shared__ uint8_t att_dyn_smem[];
-template <bool WG>
-__global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnParams p) {
-  uint8_t* fbase = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(att_dyn_smem) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = fbase;
-  uint8_t* sK[2] = {fbase + 64 * 128, fbase + 2 * 64 * 128};
-  uint8_t* sV[2] = {fbase + 3 * 64 * 128, fbase + 4 * 64 * 128};
+using T = Tile<HD>;
+constexpr int FWD_SMEM = 5 * T::BYTES + 1024;
+__global__ void __launch_bounds__(THREADS) attn_fwd_kernel(const AttnParams p) {
+  uint8_t* sQ = tile_at<HD>(0);
+  auto sK = [](int buf) { return tile_at<HD>(1 + buf); };
+  auto sV = [](int buf) { return tile_at<HD>(3 + buf); };
   __shared__ int s_red[12];
 
   const int q0 = blockIdx.x * BQ, h = blockIdx.y, b = blockIdx.z;
@@ -265,9 +119,9 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnParams 
   block_key_range(p, b, q0, s_red, klo, khi);
   const int nblk = (khi - klo + BKV - 1) / BKV;
 
-  load_tile(sQ, qp, p.ldq, q0, p.nq);
-  if (nblk > 0) { load_tile(sK[0], kp, p.ldk, klo, p.nk); load_tile(sV[0], vp, p.ldv, klo, p.nk); }
-  cp_async_commit();
+  load_tile<HD>(sQ, qp, p.ldq, q0, p.nq);
+  if (nblk > 0) { load_tile<HD>(sK(0), kp, p.ldk, klo, p.nk); load_tile<HD>(sV(0), vp, p.ldv, klo, p.nk); }
+  cp_commit();
 
   const int row_a = q0 + warp * 16 + g, row_b = row_a + 8;
   const RowInfo ra = classify_row(p, b, row_a), rb = classify_row(p, b, row_b);
@@ -277,26 +131,24 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnParams 
   for (int i = 0; i < 8; ++i) { o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f; }
   float m_a = -INFINITY, m_b = -INFINITY, l_a = 0.f, l_b = 0.f;
   const float sl2 = p.scale * LOG2E;
-  uint32_t qa[4][4];
 
   for (int j = 0; j < nblk; ++j) {
     const int buf = j & 1;
     if (j + 1 < nblk) {
-      load_tile(sK[buf ^ 1], kp, p.ldk, klo + (j + 1) * BKV, p.nk);
-      load_tile(sV[buf ^ 1], vp, p.ldv, klo + (j + 1) * BKV, p.nk);
-      cp_async_commit();
-      cp_async_wait<1>();
+      load_tile<HD>(sK(buf ^ 1), kp, p.ldk, klo + (j + 1) * BKV, p.nk);
+      load_tile<HD>(sV(buf ^ 1), vp, p.ldv, klo + (j + 1) * BKV, p.nk);
+      cp_commit();
+      cp_wait<1>();
     } else {
-      cp_async_wait<0>();
+      cp_wait<0>();
     }
-    if constexpr (WG) fence_proxy_async_smem();   // cp.async (generic proxy) -> wgmma reads
+    fence_proxy_async_smem();   // cp.async (generic proxy) -> wgmma reads
     __syncthreads();
-    if (!WG && j == 0) load_a_frags(sQ, warp * 16, qa);
 
     float s[8][4];
 #pragma unroll
     for (int i = 0; i < 8; ++i) { s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f; }
-    mma_a_tileT<WG>(s, qa, sQ, sK[buf]);
+    mma_rows_x_tileT<HD>(s, sQ, sK(buf));
 
     // mask + scale (log2 domain)
     const int key0 = klo + j * BKV;
@@ -330,65 +182,18 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnParams 
         mx_b = fmaxf(mx_b, fmaxf(s[i][2], s[i][3]));
       }
     }
-    mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 1)); mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 2));
-    mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 1)); mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 2));
-    const float mn_a = fmaxf(m_a, mx_a), mn_b = fmaxf(m_b, mx_b);
-    const float sub_a = (mn_a == -INFINITY) ? 0.f : mn_a, sub_b = (mn_b == -INFINITY) ? 0.f : mn_b;
-    const float corr_a = ex2_approx(m_a - sub_a), corr_b = ex2_approx(m_b - sub_b);  // m = -inf -> 0
-    m_a = mn_a; m_b = mn_b;
-    float rs_a = 0.f, rs_b = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      s[i][0] = ex2_approx(s[i][0] - sub_a); s[i][1] = ex2_approx(s[i][1] - sub_a);
-      s[i][2] = ex2_approx(s[i][2] - sub_b); s[i][3] = ex2_approx(s[i][3] - sub_b);
-      rs_a += s[i][0] + s[i][1]; rs_b += s[i][2] + s[i][3];
-    }
-    l_a = l_a * corr_a + rs_a; l_b = l_b * corr_b + rs_b;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { o[i][0] *= corr_a; o[i][1] *= corr_a; o[i][2] *= corr_b; o[i][3] *= corr_b; }
+    softmax_step(s, mx_a, mx_b, m_a, m_b, l_a, l_b, o);
     uint32_t pa[4][4];
     c_to_a(s, pa);
-    mma_p_tile<WG>(o, pa, sV[buf]);
+    mma_p_x_tile<HD>(o, pa, sV(buf));
     __syncthreads();
   }
-  if (nblk == 0) { cp_async_wait<0>(); }
+  if (nblk == 0) { cp_wait<0>(); }
 
-  l_a += __shfl_xor_sync(0xffffffffu, l_a, 1); l_a += __shfl_xor_sync(0xffffffffu, l_a, 2);
-  l_b += __shfl_xor_sync(0xffffffffu, l_b, 1); l_b += __shfl_xor_sync(0xffffffffu, l_b, 2);
+  l_a = quad_sum(l_a); l_b = quad_sum(l_b);
   const float inv_a = l_a > 0.f ? 1.f / l_a : 0.f, inv_b = l_b > 0.f ? 1.f / l_b : 0.f;
-  __nv_bfloat16* op = p.out + b * p.o_bs + h * HD;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int col = i * 8 + 2 * t;
-    if (row_a < p.nq) *reinterpret_cast<uint32_t*>(op + (long long)row_a * p.ldo + col) = pack_bf16x2(o[i][0] * inv_a, o[i][1] * inv_a);
-    if (row_b < p.nq) *reinterpret_cast<uint32_t*>(op + (long long)row_b * p.ldo + col) = pack_bf16x2(o[i][2] * inv_b, o[i][3] * inv_b);
-  }
-  if (p.lse != nullptr && t == 0) {
-    // log2-domain LSE of the scaled scores; rows with no mass get the sentinel 0 (P recomputes to 0 there because
-    // every score is -inf).
-    float* lp = p.lse + ((long long)b * p.heads + h) * p.nq;
-    if (row_a < p.nq) lp[row_a] = l_a > 0.f ? m_a + log2f(l_a) : 0.f;
-    if (row_b < p.nq) lp[row_b] = l_b > 0.f ? m_b + log2f(l_b) : 0.f;
-  }
-}
-
-// ================================================================ backward: delta = rowsum(dO * O)
-__global__ void attn_delta_kernel(const AttnParams p) {
-  const int warps_per_block = blockDim.x >> 5;
-  const long long row = (long long)blockIdx.x * warps_per_block + (threadIdx.x >> 5);  // over batch*heads*nq
-  const long long total = (long long)p.batch * p.heads * p.nq;
-  if (row >= total) return;
-  const int lane = threadIdx.x & 31;
-  const int qi = (int)(row % p.nq);
-  const int h = (int)((row / p.nq) % p.heads);
-  const int b = (int)(row / ((long long)p.nq * p.heads));
-  const __nv_bfloat16* op = p.o + b * p.o_bs + (long long)qi * p.ldo + h * HD;
-  const __nv_bfloat16* dop = p.d_o + b * p.o_bs + (long long)qi * p.ldo + h * HD;
-  const uint32_t a = *reinterpret_cast<const uint32_t*>(op + 2 * lane);
-  const uint32_t d = *reinterpret_cast<const uint32_t*>(dop + 2 * lane);
-  float v = bf16_lo(a) * bf16_lo(d) + bf16_hi(a) * bf16_hi(d);
-  v = warp_sum(v);
-  if (lane == 0) p.delta[row] = v;
+  store_rows(p.out + b * p.o_bs + h * HD, p.ldo, o, inv_a, inv_b, row_a, row_b, p.nq, t);
+  if (p.lse != nullptr && t == 0) store_lse(p.lse + ((long long)b * p.heads + h) * p.nq, m_a, l_a, m_b, l_b, row_a, row_b, p.nq);
 }
 
 // Recompute P (C layout, rows = queries) for one 16x64 tile given raw S = Q K^T.
@@ -425,15 +230,13 @@ __device__ __forceinline__ void recompute_p(const AttnParams& p, float (&s)[8][4
 }
 
 // ================================================================ backward: dQ  (CTA = 64 queries, loop over key tiles)
-constexpr int BWD_SMEM = 6 * 64 * 128 + 1024;  // six 8 KiB tiles + alignment slack
+constexpr int BWD_SMEM = 6 * T::BYTES + 1024;
 
-template <bool WG>
-__global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnParams p) {
-  uint8_t* base_ = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(att_dyn_smem) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = base_;
-  uint8_t* sdO = base_ + 8192;
-  uint8_t* sK[2] = {base_ + 2 * 8192, base_ + 3 * 8192};
-  uint8_t* sV[2] = {base_ + 4 * 8192, base_ + 5 * 8192};
+__global__ void __launch_bounds__(THREADS) attn_bwd_dq_kernel(const AttnParams p) {
+  uint8_t* sQ = tile_at<HD>(0);
+  uint8_t* sdO = tile_at<HD>(1);
+  auto sK = [](int buf) { return tile_at<HD>(2 + buf); };
+  auto sV = [](int buf) { return tile_at<HD>(4 + buf); };
   __shared__ int s_red[12];
 
   const int q0 = blockIdx.x * BQ, h = blockIdx.y, b = blockIdx.z;
@@ -447,10 +250,10 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
   block_key_range(p, b, q0, s_red, klo, khi);
   const int nblk = (khi - klo + BKV - 1) / BKV;
 
-  load_tile(sQ, qp, p.ldq, q0, p.nq);
-  load_tile(sdO, dop, p.ldo, q0, p.nq);
-  if (nblk > 0) { load_tile(sK[0], kp, p.ldk, klo, p.nk); load_tile(sV[0], vp, p.ldv, klo, p.nk); }
-  cp_async_commit();
+  load_tile<HD>(sQ, qp, p.ldq, q0, p.nq);
+  load_tile<HD>(sdO, dop, p.ldo, q0, p.nq);
+  if (nblk > 0) { load_tile<HD>(sK(0), kp, p.ldk, klo, p.nk); load_tile<HD>(sV(0), vp, p.ldv, klo, p.nk); }
+  cp_commit();
 
   const int row_a = q0 + warp * 16 + g, row_b = row_a + 8;
   const RowInfo ra = classify_row(p, b, row_a), rb = classify_row(p, b, row_b);
@@ -462,27 +265,25 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
   float dq[8][4];
 #pragma unroll
   for (int i = 0; i < 8; ++i) { dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f; }
-  uint32_t qa[4][4], doa[4][4];
 
   for (int j = 0; j < nblk; ++j) {
     const int buf = j & 1;
     if (j + 1 < nblk) {
-      load_tile(sK[buf ^ 1], kp, p.ldk, klo + (j + 1) * BKV, p.nk);
-      load_tile(sV[buf ^ 1], vp, p.ldv, klo + (j + 1) * BKV, p.nk);
-      cp_async_commit();
-      cp_async_wait<1>();
+      load_tile<HD>(sK(buf ^ 1), kp, p.ldk, klo + (j + 1) * BKV, p.nk);
+      load_tile<HD>(sV(buf ^ 1), vp, p.ldv, klo + (j + 1) * BKV, p.nk);
+      cp_commit();
+      cp_wait<1>();
     } else {
-      cp_async_wait<0>();
+      cp_wait<0>();
     }
-    if constexpr (WG) fence_proxy_async_smem();   // cp.async (generic proxy) -> wgmma reads
+    fence_proxy_async_smem();   // cp.async (generic proxy) -> wgmma reads
     __syncthreads();
-    if (!WG && j == 0) { load_a_frags(sQ, warp * 16, qa); load_a_frags(sdO, warp * 16, doa); }
 
     float s[8][4], dpv[8][4];
 #pragma unroll
     for (int i = 0; i < 8; ++i) { s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f; dpv[i][0] = dpv[i][1] = dpv[i][2] = dpv[i][3] = 0.f; }
-    mma_a_tileT<WG>(s, qa, sQ, sK[buf]);      // S  = Q K^T
-    mma_a_tileT<WG>(dpv, doa, sdO, sV[buf]);   // dP = dO V^T
+    mma_rows_x_tileT<HD>(s, sQ, sK(buf));      // S  = Q K^T
+    mma_rows_x_tileT<HD>(dpv, sdO, sV(buf));   // dP = dO V^T
     recompute_p(p, s, ra, rb, lse_a, lse_b, klo + j * BKV, t);
     const float ga = ra.kind == 2 ? 0.f : p.scale, gb = rb.kind == 2 ? 0.f : p.scale;
 #pragma unroll
@@ -492,30 +293,22 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
     }
     uint32_t dsa[4][4];
     c_to_a(s, dsa);
-    mma_p_tile<WG>(dq, dsa, sK[buf]);     // dQ += dS K
+    mma_p_x_tile<HD>(dq, dsa, sK(buf));     // dQ += dS K
     __syncthreads();
   }
-  if (nblk == 0) { cp_async_wait<0>(); }
+  if (nblk == 0) { cp_wait<0>(); }
 
-  __nv_bfloat16* dqp = p.dq + b * p.dq_bs + h * HD;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int col = i * 8 + 2 * t;
-    if (row_a < p.nq) *reinterpret_cast<uint32_t*>(dqp + (long long)row_a * p.lddq + col) = pack_bf16x2(dq[i][0], dq[i][1]);
-    if (row_b < p.nq) *reinterpret_cast<uint32_t*>(dqp + (long long)row_b * p.lddq + col) = pack_bf16x2(dq[i][2], dq[i][3]);
-  }
+  store_rows(p.dq + b * p.dq_bs + h * HD, p.lddq, dq, 1.f, 1.f, row_a, row_b, p.nq, t);
 }
 
 // ================================================================ backward: dK, dV (CTA = 64 keys, loop over query tiles)
 // Works on transposed tiles: S^T = K Q^T (rows = keys), so P^T / dS^T are directly the A operands of
 // dV += P^T dO and dK += dS^T Q.
-template <bool WG>
-__global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const AttnParams p) {
-  uint8_t* base_ = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(att_dyn_smem) + 1023) & ~uintptr_t(1023));
-  uint8_t* sK = base_;
-  uint8_t* sV = base_ + 8192;
-  uint8_t* sQ[2] = {base_ + 2 * 8192, base_ + 3 * 8192};
-  uint8_t* sdO[2] = {base_ + 4 * 8192, base_ + 5 * 8192};
+__global__ void __launch_bounds__(THREADS) attn_bwd_dkv_kernel(const AttnParams p) {
+  uint8_t* sK = tile_at<HD>(0);
+  uint8_t* sV = tile_at<HD>(1);
+  auto sQ = [](int buf) { return tile_at<HD>(2 + buf); };
+  auto sdO = [](int buf) { return tile_at<HD>(4 + buf); };
   __shared__ float s_lse[2][BQ], s_del[2][BQ];
   __shared__ int s_tt[2][BQ], s_kind[2][BQ];
 
@@ -539,11 +332,11 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const AttnPar
     }
   };
 
-  load_tile(sK, kp, p.ldk, k0, p.nk);
-  load_tile(sV, vp, p.ldv, k0, p.nk);
-  load_tile(sQ[0], qp, p.ldq, 0, p.nq);
-  load_tile(sdO[0], dop, p.ldo, 0, p.nq);
-  cp_async_commit();
+  load_tile<HD>(sK, kp, p.ldk, k0, p.nk);
+  load_tile<HD>(sV, vp, p.ldv, k0, p.nk);
+  load_tile<HD>(sQ(0), qp, p.ldq, 0, p.nq);
+  load_tile<HD>(sdO(0), dop, p.ldo, 0, p.nq);
+  cp_commit();
   stage_rows(0, 0);
 
   float dk[8][4], dv[8][4];
@@ -557,15 +350,15 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const AttnPar
   for (int qb = 0; qb < nqb; ++qb) {
     const int buf = qb & 1;
     if (qb + 1 < nqb) {
-      load_tile(sQ[buf ^ 1], qp, p.ldq, (qb + 1) * BQ, p.nq);
-      load_tile(sdO[buf ^ 1], dop, p.ldo, (qb + 1) * BQ, p.nq);
-      cp_async_commit();
+      load_tile<HD>(sQ(buf ^ 1), qp, p.ldq, (qb + 1) * BQ, p.nq);
+      load_tile<HD>(sdO(buf ^ 1), dop, p.ldo, (qb + 1) * BQ, p.nq);
+      cp_commit();
       stage_rows(buf ^ 1, qb + 1);
-      cp_async_wait<1>();
+      cp_wait<1>();
     } else {
-      cp_async_wait<0>();
+      cp_wait<0>();
     }
-    if constexpr (WG) fence_proxy_async_smem();   // cp.async (generic proxy) -> wgmma reads
+    fence_proxy_async_smem();   // cp.async (generic proxy) -> wgmma reads
     __syncthreads();
     {
       // skip (query block, key block) pairs the media mask rules out entirely
@@ -584,13 +377,8 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const AttnPar
     float st[8][4], dpt[8][4];
 #pragma unroll
     for (int i = 0; i < 8; ++i) { st[i][0] = st[i][1] = st[i][2] = st[i][3] = 0.f; dpt[i][0] = dpt[i][1] = dpt[i][2] = dpt[i][3] = 0.f; }
-    {
-      uint32_t fa[4][4];              // A fragments are re-read from smem each time: keeps the kernel under 255 regs
-      if (!WG) load_a_frags(sK, warp * 16, fa);
-      mma_a_tileT<WG>(st, fa, sK, sQ[buf]);     // S^T  = K Q^T   [16 keys x 64 queries]
-      if (!WG) load_a_frags(sV, warp * 16, fa);
-      mma_a_tileT<WG>(dpt, fa, sV, sdO[buf]);   // dP^T = V dO^T
-    }
+    mma_rows_x_tileT<HD>(st, sK, sQ(buf));     // S^T  = K Q^T   [16 keys x 64 queries]
+    mma_rows_x_tileT<HD>(dpt, sV, sdO(buf));   // dP^T = V dO^T
     float dst[8][4];
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -608,28 +396,14 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const AttnPar
     uint32_t pa[4][4], dsa[4][4];
     c_to_a(st, pa);
     c_to_a(dst, dsa);
-    mma_p_tile<WG>(dv, pa, sdO[buf]);     // dV += P^T dO
-    mma_p_tile<WG>(dk, dsa, sQ[buf]);     // dK += dS^T Q
+    mma_p_x_tile<HD>(dv, pa, sdO(buf));     // dV += P^T dO
+    mma_p_x_tile<HD>(dk, dsa, sQ(buf));     // dK += dS^T Q
     __syncthreads();
   }
 
-  __nv_bfloat16* dkp = p.dk + b * p.dk_bs + h * HD;
-  __nv_bfloat16* dvp = p.dv + b * p.dv_bs + h * HD;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int col = i * 8 + 2 * t;
-    if (key_a < p.nk) {
-      *reinterpret_cast<uint32_t*>(dkp + (long long)key_a * p.lddk + col) = pack_bf16x2(dk[i][0], dk[i][1]);
-      *reinterpret_cast<uint32_t*>(dvp + (long long)key_a * p.lddv + col) = pack_bf16x2(dv[i][0], dv[i][1]);
-    }
-    if (key_b < p.nk) {
-      *reinterpret_cast<uint32_t*>(dkp + (long long)key_b * p.lddk + col) = pack_bf16x2(dk[i][2], dk[i][3]);
-      *reinterpret_cast<uint32_t*>(dvp + (long long)key_b * p.lddv + col) = pack_bf16x2(dv[i][2], dv[i][3]);
-    }
-  }
+  store_rows(p.dk + b * p.dk_bs + h * HD, p.lddk, dk, 1.f, 1.f, key_a, key_b, p.nk, t);
+  store_rows(p.dv + b * p.dv_bs + h * HD, p.lddv, dv, 1.f, 1.f, key_a, key_b, p.nk, t);
 }
-
-static bool aligned(const void* ptr, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(ptr) & (bytes - 1)) == 0; }
 
 // q/k/v/o/dO are read (and o written) 16 bytes at a time per row and 32 bits at a time by the delta kernel; dq/dk/dv
 // are written 32 bits at a time; lse/delta/text_time are f32/int32 arrays.  Called before any CUDA call.
@@ -674,14 +448,8 @@ extern "C" int ofk_attn_fwd(const void* q, const void* k, const void* v, void* o
   if (!q || !k || !v || !o) return ofk_set_error(OFK_ERR_ARG, "attention: null pointer");
   if (int rc = check_common(p, false)) return rc;
   dim3 grid((nq + BQ - 1) / BQ, heads, batch);
-  if (ofk_attn_use_wgmma()) {
-    attn_fwd_kernel<true><<<grid, ATT_THREADS, FWD_SMEM, (cudaStream_t)stream_>>>(p);
-    OFK_CHECK_LAUNCH();
-    ofk_attn_count_wgmma();
-  } else {
-    attn_fwd_kernel<false><<<grid, ATT_THREADS, FWD_SMEM, (cudaStream_t)stream_>>>(p);
-    OFK_CHECK_LAUNCH();
-  }
+  attn_fwd_kernel<<<grid, THREADS, FWD_SMEM, (cudaStream_t)stream_>>>(p);
+  OFK_CHECK_LAUNCH();
   return 0;
 }
 
@@ -706,29 +474,19 @@ extern "C" int ofk_attn_bwd(const void* q, const void* k, const void* v, const v
   if (int rc = check_common(p, true)) return rc;
   cudaStream_t stream = (cudaStream_t)stream_;
   const long long rows = (long long)batch * heads * nq;
-  attn_delta_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(p);
+  delta_kernel<HD><<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(p.o, p.d_o, p.delta, batch, heads, nq, p.o_bs, p.ldo);
   OFK_CHECK_LAUNCH();
   dim3 gq((nq + BQ - 1) / BQ, heads, batch);
   static bool attr_done = false;
   if (!attr_done) {
-    cudaFuncSetAttribute(attn_bwd_dq_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
-    cudaFuncSetAttribute(attn_bwd_dkv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
-    cudaFuncSetAttribute(attn_bwd_dq_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
-    cudaFuncSetAttribute(attn_bwd_dkv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
+    cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
+    cudaFuncSetAttribute(attn_bwd_dkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
     attr_done = true;
   }
   dim3 gk((nk + BKV - 1) / BKV, heads, batch);
-  if (ofk_attn_use_wgmma()) {
-    attn_bwd_dq_kernel<true><<<gq, ATT_THREADS, BWD_SMEM, stream>>>(p);
-    OFK_CHECK_LAUNCH();
-    attn_bwd_dkv_kernel<true><<<gk, ATT_THREADS, BWD_SMEM, stream>>>(p);
-    OFK_CHECK_LAUNCH();
-    ofk_attn_count_wgmma();
-  } else {
-    attn_bwd_dq_kernel<false><<<gq, ATT_THREADS, BWD_SMEM, stream>>>(p);
-    OFK_CHECK_LAUNCH();
-    attn_bwd_dkv_kernel<false><<<gk, ATT_THREADS, BWD_SMEM, stream>>>(p);
-    OFK_CHECK_LAUNCH();
-  }
+  attn_bwd_dq_kernel<<<gq, THREADS, BWD_SMEM, stream>>>(p);
+  OFK_CHECK_LAUNCH();
+  attn_bwd_dkv_kernel<<<gk, THREADS, BWD_SMEM, stream>>>(p);
+  OFK_CHECK_LAUNCH();
   return 0;
 }

@@ -5,10 +5,6 @@
 // Records the message returned by ofk_last_error() (thread-local) and returns `code`.
 int ofk_set_error(int code, const char* msg);
 void ofk_count_launch();
-// Attention: true unless the mma.sync kernels were forced (ofk_attn_force_legacy / OFK_ATTN_LEGACY=1); every entry-point
-// call served by the wgmma kernels is counted (ofk_attn_tc_launch_count).
-bool ofk_attn_use_wgmma();
-void ofk_attn_count_wgmma();
 
 #define OFK_CHECK_LAUNCH()                                                        \
   do {                                                                            \

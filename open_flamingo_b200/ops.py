@@ -183,17 +183,6 @@ def _dense_mask_slopes(mask, slopes, pure_causal_flag, B, heads, nq, nk):
         raise ValueError("pure_causal_flag must be an int32 device tensor")
 
 
-def attn_force_legacy(on):
-    """A/B switch: True = the mma.sync attention kernels, False = the wgmma kernels (the default).  Returns the
-    previous setting."""
-    return bool(L.lib().ofk_attn_force_legacy(int(bool(on))))
-
-
-def attn_tc_launch_count():
-    """Attention calls (forward or backward) served by the wgmma kernels so far."""
-    return int(L.lib().ofk_attn_tc_launch_count())
-
-
 def attn_fwd(q, k, v, heads, scale, *, mask_mode=L.MASK_NONE, text_time=None, keys_per_media=64, out=None,
              want_lse=True):
     """q: [B, nq, heads*64] (may be a column-slice view), k/v: [B, nk, heads*64].  Returns (o, lse)."""

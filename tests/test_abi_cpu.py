@@ -23,7 +23,7 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, name), f"{name} declared in ofk.h but not exported by libofk.so"
     assert sorted(_lib.exported_symbols()) == declared, "ctypes signature table and ofk.h disagree"
     loaded = _lib.lib()
-    assert loaded.ofk_abi_version() == 3
+    assert loaded.ofk_abi_version() == 4
     assert isinstance(_lib.launch_count(), int)
 
 
@@ -74,8 +74,7 @@ def _sass_by_kernel():
 
 def test_hot_kernels_are_wgmma_and_tma_in_the_shipped_binary():
     """Static proof, on the .so the tests load: every GEMM kernel issues warpgroup MMAs (HGMMA) on operands staged by TMA
-    (UTMALDG), with no mma.sync (HMMA) path inside; the default attention cores issue wgmma and no mma.sync, the
-    reference ones mma.sync."""
+    (UTMALDG), with no mma.sync (HMMA) path inside; every attention core issues wgmma and no mma.sync."""
     kernels = _sass_by_kernel()
     assert len(kernels) > 40
     gemms = {k: v for k, v in kernels.items() if "gemm_kernel" in k}
@@ -86,11 +85,7 @@ def test_hot_kernels_are_wgmma_and_tma_in_the_shipped_binary():
         assert "HMMA" not in ops_, f"{k}: mma.sync inside a wgmma kernel"
     attn = {k: v for k, v in kernels.items() if re.search(r"attn_fwd_kernel|attn_bwd_dq_kernel|attn_bwd_dkv_kernel|"
                                                           r"dense\d+fwd_kernel|dense\d+bwd_dq_kernel|dense\d+bwd_dkv_kernel", k)}
-    wg = {k: v for k, v in attn.items() if "Lb1E" in k}      # template flag WG = true: the default path
-    ref = {k: v for k, v in attn.items() if "Lb0E" in k}     # the mma.sync A/B reference
-    assert len(wg) == 3 + 3 * 2 and len(ref) == 3 + 3 * 2, sorted(attn)   # media cores + dense cores for head_dim 64 and 128
-    for k, ops_ in wg.items():
-        assert "HGMMA" in ops_, f"{k}: default attention core without wgmma"
+    assert len(attn) == 3 + 3 * 2, sorted(attn)   # media cores + dense cores for head_dim 64 and 128
+    for k, ops_ in attn.items():
+        assert "HGMMA" in ops_, f"{k}: attention core without wgmma"
         assert "HMMA" not in ops_, f"{k}: mma.sync inside a wgmma attention core"
-    for k, ops_ in ref.items():
-        assert "HMMA" in ops_, f"{k}: reference attention core without mma.sync"

@@ -1,8 +1,7 @@
 """GPU: the training attention kernels against a float64 restatement of their semantics, with per-element bounds.
 
 Entry points: ofk_attn_fwd / ofk_attn_bwd (media rules: Perceiver, gated cross-attention, ViT) and ofk_attn_dense_fwd /
-ofk_attn_dense_bwd (MPT blocks, including the chunked-prefill call with nq < nk over the KV cache).  Every case runs on the
-default wgmma kernels and on the mma.sync kernels (ofk_attn_force_legacy), and the launch counter proves which served it.
+ofk_attn_dense_bwd (MPT blocks, including the chunked-prefill call with nq < nk over the KV cache).
 
 Semantics restated (computed in float64 on the GPU from the same bf16 inputs):
   media  (helpers.py:190-232): key allowed when text_time == key // kpm + 1 (mode 1) or >= (mode 2); a row with no
@@ -59,13 +58,6 @@ def ops():
 def lib():
     from open_flamingo_b200 import _lib
     return _lib
-
-
-@pytest.fixture(params=[False, True], ids=["wgmma", "mma_sync"])
-def legacy(request, ops):
-    prev = ops.attn_force_legacy(request.param)
-    yield request.param
-    ops.attn_force_legacy(prev)
 
 
 # ------------------------------------------------------------------ NaN-surrounded views and canary windows
@@ -242,11 +234,6 @@ def check_bwd(R, o, dq, dk, dv, what):
         assert bool((heads_split(dv, H, hd)[dead] == 0).all()), f"{what}: unreachable keys have nonzero dv"
 
 
-def _count(ops, legacy, n0, calls, what):
-    got = ops.attn_tc_launch_count() - n0
-    assert got == (0 if legacy else calls), f"{what}: {got} calls on the wgmma kernels, expected {0 if legacy else calls}"
-
-
 # ------------------------------------------------------------------ media rules
 def media_allowed(tt, nk, kpm, mode):
     B, nq = tt.shape
@@ -332,13 +319,12 @@ def _media_case(case, seed=0):
 
 
 @pytest.mark.parametrize("case", MEDIA_CASES + BIG, ids=lambda c: "-".join(map(str, c)))
-def test_media_attention_against_float64(ops, legacy, case):
+def test_media_attention_against_float64(ops, case):
     B, heads, nq, nk, mode, kpm, _ = case
     D = heads * 64
     scale, tt, allowed, zero, q, k, v, d_o = _media_case(case)
     qw, kv_k, kv_v, d_o16 = place_inputs(q, k, v, d_o)
     ow = Window(B, nq, D, r0=1, c0=64, pad=2, extra=8)
-    n0 = ops.attn_tc_launch_count()
     o, lse = ops.attn_fwd(qw, kv_k, kv_v, heads, scale, mask_mode=mode, text_time=tt, keys_per_media=kpm, out=ow.view)
     o2, none = ops.attn_fwd(qw, kv_k, kv_v, heads, scale, mask_mode=mode, text_time=tt, keys_per_media=kpm,
                             want_lse=False)
@@ -351,12 +337,11 @@ def test_media_attention_against_float64(ops, legacy, case):
     ops.attn_bwd(qw, kv_k, kv_v, o, dow.view, lse, heads, scale, mask_mode=mode, text_time=tt, keys_per_media=kpm,
                  dq=dqw.view, dk=dkw.view, dv=dvw.view)
     torch.cuda.synchronize()
-    _count(ops, legacy, n0, 3, "media")
     assert none is None and torch.equal(o, o2), "output without the LSE differs from the output with it"
     for w, name in ((ow, "o"), (dqw, "dq"), (dkw, "dk"), (dvw, "dv")):
         w.check(name)
     R = reference(qw, kv_k, kv_v, d_o16, heads, 64, scale, allowed, zero, uniform_lse=lambda n: math.log2(n))
-    what = f"media {case} {'mma.sync' if legacy else 'wgmma'}"
+    what = f"media {case}"
     check_fwd(R, o, lse, 2.0 ** -8, what)
     check_bwd(R, o, dqw.view, dkw.view, dvw.view, what)
 
@@ -426,7 +411,7 @@ DENSE_CASES.append((3, 4, 128, 63, 200, "left_pad", True, False, True))
 
 
 @pytest.mark.parametrize("case", DENSE_CASES, ids=lambda c: "-".join(map(str, c)))
-def test_dense_attention_against_float64(ops, lib, legacy, case):
+def test_dense_attention_against_float64(ops, lib, case):
     B, heads, hd, nq, nk, kind, alibi, plant, bwd = case
     D = heads * hd
     scale = hd ** -0.5
@@ -448,11 +433,9 @@ def test_dense_attention_against_float64(ops, lib, legacy, case):
     causal = mask is None and kind != "flag"
     ow = Window(B, nq, D, r0=2, c0=8, pad=1, extra=64)
     lsew = Window(1, 1, B * heads * nq, c0=4, extra=4, dtype=f32)
-    n0 = ops.attn_tc_launch_count()
     dense_fwd_ctypes(lib, qw, kv_k, kv_v, heads, hd, scale, causal, mask8, slopes, flag, ow.view, lsew.view)
     o2, _ = ops.attn_dense_fwd(qw, kv_k, kv_v, heads, hd, scale, causal=causal, mask=mask8, slopes=slopes,
                                pure_causal_flag=flag, want_lse=False)
-    calls = 2
     o, lse = ow.view, lsew.view.reshape(B, heads, nq)
     if bwd:
         dow = Window(B, nq, D, r0=2, c0=8, pad=1, extra=64)
@@ -462,15 +445,13 @@ def test_dense_attention_against_float64(ops, lib, legacy, case):
         dvw = Window(B, nk, D, r0=3, c0=0, pad=0, extra=8)
         ops.attn_dense_bwd(qw, kv_k, kv_v, o, dow.view, lse, heads, hd, scale, causal=causal, mask=mask8,
                            slopes=slopes, pure_causal_flag=flag, dq=dqw.view, dk=dkw.view, dv=dvw.view)
-        calls += 1
     torch.cuda.synchronize()
-    _count(ops, legacy, n0, calls, "dense")
     assert torch.equal(o, o2), "output without the LSE differs from the output with it"
     ow.check("o")
     lsew.check("lse")
     R = reference(qw, kv_k, kv_v, d_o16, heads, hd, scale, ~masked, slopes=slopes,
                   uniform_lse=lambda n: MASKED_LOG2 + math.log2(n))
-    what = f"dense {case} {'mma.sync' if legacy else 'wgmma'}"
+    what = f"dense {case}"
     check_fwd(R, o, lse, 2.0 ** -16, what)
     if bwd:
         for w, name in ((dqw, "dq"), (dkw, "dk"), (dvw, "dv")):
@@ -500,7 +481,7 @@ def _assert_same(a, b, what):
 
 @pytest.mark.parametrize("case", [(3, 8, 129, 240, 1, 80, True), (3, 4, 65, 257, 0, 64, False),
                                   (3, 4, 129, 192, 2, 64, True)], ids=lambda c: "-".join(map(str, c)))
-def test_media_repeatable_and_independent_of_other_batches_and_heads(ops, legacy, case):
+def test_media_repeatable_and_independent_of_other_batches_and_heads(ops, case):
     B, heads, nq, nk, mode, kpm, _ = case
     scale, tt, _, _, q, k, v, d_o = _media_case(case, seed=1)
     q, k, v, d_o = (t.to(bf16) for t in (q, k, v, d_o))
@@ -520,7 +501,7 @@ def test_media_repeatable_and_independent_of_other_batches_and_heads(ops, legacy
 
 @pytest.mark.parametrize("shape", [(2, 4, 128, 129, 129), (2, 2, 64, 63, 200), (3, 2, 128, 65, 1000)],
                          ids=lambda c: "-".join(map(str, c)))
-def test_dense_flag_repeatable_and_independent(ops, legacy, shape):
+def test_dense_flag_repeatable_and_independent(ops, shape):
     """pure_causal_flag = 1 over garbage mask bytes gives the bits of causal=True without a mask (nq <= nk); with the flag
     at 0 the same bytes are honoured; launches repeat bit for bit; one (batch, head) computed alone gives the same bits."""
     B, heads, hd, nq, nk = shape

@@ -1,8 +1,6 @@
-"""GPU: the wgmma attention kernels are the DEFAULT path of ofk_attn_fwd / ofk_attn_bwd / ofk_attn_dense_fwd /
-ofk_attn_dense_bwd.  Each case is checked three ways: against a plain fp32 torch restatement of the reference semantics
-(helpers.py:190-232 for the media rules; HF MptAttention for the dense rules), against the mma.sync kernels run on the
-same inputs (ofk_attn_force_legacy), and by the launch counter that proves the wgmma kernels -- not the mma.sync
-ones -- served the default call."""
+"""GPU: the wgmma attention kernels behind ofk_attn_fwd / ofk_attn_bwd / ofk_attn_dense_fwd / ofk_attn_dense_bwd against
+a plain fp32 torch restatement of the reference semantics (helpers.py:190-232 for the media rules; HF MptAttention for
+the dense rules)."""
 import pytest
 import torch
 
@@ -26,7 +24,7 @@ def _media_run(ops, q, k, v, d_o, heads, scale, mode, tt, kpm):
 
 
 @pytest.mark.parametrize("case", CASES)
-def test_media_attention_tc_vs_reference_and_legacy(ops, case):
+def test_media_attention_tc_vs_reference(ops, case):
     B, heads, nq, nk, mode, kpm = case
     torch.manual_seed(11)
     inner = heads * 64
@@ -40,24 +38,9 @@ def test_media_attention_tc_vs_reference_and_legacy(ops, case):
         tt = make_tt(B, nq, nk // kpm, mode, 7).cuda()
         if nq == 1:
             tt[:] = nk // kpm
-    n0 = ops.attn_tc_launch_count()
     o, lse, dq, dk, dv = _media_run(ops, q, k, v, d_o, heads, scale, mode, tt, kpm)
-    want = 2   # the forward and the backward call
-    assert ops.attn_tc_launch_count() - n0 == want, "default attention path is not the wgmma one"
-    prev = ops.attn_force_legacy(True)
-    try:
-        o2, lse2, dq2, dk2, dv2 = _media_run(ops, q, k, v, d_o, heads, scale, mode, tt, kpm)
-    finally:
-        ops.attn_force_legacy(prev)
-    assert ops.attn_tc_launch_count() - n0 == want
     for t in (o, lse, dq, dk, dv):
         assert torch.isfinite(t.float()).all()
-    # the two implementations differ only in fp32 summation order and one bf16 rounding of P / dS
-    close(o, o2, 1e-2, "o wgmma vs mma.sync")
-    assert (lse - lse2).abs().max().item() <= 2e-3 * (1 + lse2.abs().max().item())
-    close(dq, dq2, 2e-2, "dq wgmma vs mma.sync")
-    close(dk, dk2, 2e-2, "dk wgmma vs mma.sync")
-    close(dv, dv2, 2e-2, "dv wgmma vs mma.sync")
     # fp32 reference
     qr, kr, vr = (t.float().requires_grad_(True) for t in (q, k, v))
     ref = ref_attention(qr, kr, vr, heads, scale, mode, tt, kpm)
@@ -103,9 +86,10 @@ def test_vit_tail_rows_split(ops):
     qkv = torch.randn(B, n, 3 * heads * 64, device="cuda").to(bf16)
     D = heads * 64
     q, k, v = qkv[..., :D], qkv[..., D:2 * D], qkv[..., 2 * D:]
-    n0 = ops.attn_tc_launch_count()
+    from open_flamingo_b200 import _lib
+    n0 = _lib.launch_count()
     o_split, _ = ops.attn_fwd(q, k, v, heads, 0.125, want_lse=False)
-    assert ops.attn_tc_launch_count() - n0 == 1
+    assert _lib.launch_count() - n0 == 1   # one forward-core launch, no separate LSE pass
     o_full, _ = ops.attn_fwd(q, k, v, heads, 0.125, want_lse=True)
     torch.cuda.synchronize()
     close(o_split, ref_attention(q, k, v, heads, 0.125, 0, None, 64), 2e-2, "vit split vs fp32")
@@ -159,7 +143,7 @@ DENSE_CASES = [
 
 
 @pytest.mark.parametrize("case", DENSE_CASES)
-def test_dense_attention_tc_vs_reference_and_legacy(ops, case):
+def test_dense_attention_tc_vs_reference(ops, case):
     B, heads, hd, T, kind, alibi = case
     torch.manual_seed(13)
     D = heads * hd
@@ -178,18 +162,8 @@ def test_dense_attention_tc_vs_reference_and_legacy(ops, case):
         torch.cuda.synchronize()
         return o, lse, dqkv
 
-    n0 = ops.attn_tc_launch_count()
     o, lse, dqkv = run()
-    assert ops.attn_tc_launch_count() - n0 == 2, "default dense attention path is not the wgmma one"
-    prev = ops.attn_force_legacy(True)
-    try:
-        o2, lse2, dqkv2 = run()
-    finally:
-        ops.attn_force_legacy(prev)
     assert torch.isfinite(o.float()).all() and torch.isfinite(dqkv.float()).all()
-    close(o, o2, 1e-2, "dense o wgmma vs mma.sync")
-    assert (lse - lse2).abs().max().item() <= 2e-3 * (1 + lse2.abs().max().item())
-    close(dqkv, dqkv2, 2e-2, "dense dqkv wgmma vs mma.sync")
     qr, kr, vr = (t.float().requires_grad_(True) for t in (q, k, v))
     ref = ref_dense(qr, kr, vr, heads, hd, scale, causal, mask, slopes)
     ref.backward(d_o.float())
