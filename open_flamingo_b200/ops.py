@@ -173,6 +173,39 @@ def _attn_text_time(text_time, B, nq):
     return text_time.contiguous()
 
 
+def _attn_strides(*named):
+    """(batch stride, row stride) of each (tensor, name) pair, flattened in order."""
+    return tuple(st for t, name in named for st in _bstride_ld(t, name))
+
+
+def _attn_fwd_outputs(q, B, heads, nq, inner, out, want_lse):
+    """o (allocated unless given) and lse (None unless wanted) of a forward call."""
+    if out is None:
+        out = torch.empty((B, nq, inner), device=q.device, dtype=bf16)
+    _attn_rows(out, "out", (B, nq, inner))
+    lse = torch.empty((B, heads, nq), device=q.device, dtype=f32) if want_lse else None
+    return out, lse
+
+
+def _attn_bwd_buffers(q, k, v, o, d_o, lse, heads, inner, dq, dk, dv):
+    """Checks shared by the backward wrappers; allocates the gradients not given and delta.
+    Returns (B, nq, nk, dq, dk, dv, delta)."""
+    B, nq, nk = _attn_qkv(q, k, v, inner)
+    _attn_rows(o, "o", (B, nq, inner))
+    _attn_rows(d_o, "d_o", (B, nq, inner))
+    if d_o.stride() != o.stride():
+        raise ValueError("d_o must have the same strides as o")
+    _attn_lse(lse, B, heads, nq)
+    grads = []
+    for t, name, n in ((dq, "dq", nq), (dk, "dk", nk), (dv, "dv", nk)):
+        if t is None:
+            t = torch.empty((B, n, inner), device=q.device, dtype=bf16)
+        _attn_rows(t, name, (B, n, inner))
+        grads.append(t)
+    delta = torch.empty((B, heads, nq), device=q.device, dtype=f32)
+    return (B, nq, nk, *grads, delta)
+
+
 def _dense_mask_slopes(mask, slopes, pure_causal_flag, B, heads, nq, nk):
     # the kernel indexes mask as a contiguous [B, nq, nk] byte array and reads slopes[h]
     if mask is not None and (tuple(mask.shape) != (B, nq, nk) or not mask.is_contiguous() or mask.element_size() != 1):
@@ -188,19 +221,12 @@ def attn_fwd(q, k, v, heads, scale, *, mask_mode=L.MASK_NONE, text_time=None, ke
     """q: [B, nq, heads*64] (may be a column-slice view), k/v: [B, nk, heads*64].  Returns (o, lse)."""
     L.require_cuda(q, k, v, out, text_time)
     B, nq, nk = _attn_qkv(q, k, v, heads * 64)
-    if out is None:
-        out = torch.empty((B, nq, heads * 64), device=q.device, dtype=bf16)
-    _attn_rows(out, "out", (B, nq, heads * 64))
-    lse = torch.empty((B, heads, nq), device=q.device, dtype=f32) if want_lse else None
-    qb, ldq = _bstride_ld(q, "q")
-    kb, ldk = _bstride_ld(k, "k")
-    vb, ldv = _bstride_ld(v, "v")
-    ob, ldo = _bstride_ld(out, "out")
+    out, lse = _attn_fwd_outputs(q, B, heads, nq, heads * 64, out, want_lse)
+    strides = _attn_strides((q, "q"), (k, "k"), (v, "v"), (out, "out"))
     if mask_mode != L.MASK_NONE:
         text_time = _attn_text_time(text_time, B, nq)
     L.check(L.lib().ofk_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), L.ptr(lse), B, heads, nq, nk,
-                                 qb, ldq, kb, ldk, vb, ldv, ob, ldo, scale, mask_mode, L.ptr(text_time), keys_per_media,
-                                 L.stream_ptr()))
+                                 *strides, scale, mask_mode, L.ptr(text_time), keys_per_media, L.stream_ptr()))
     return out, lse
 
 
@@ -208,36 +234,13 @@ def attn_bwd(q, k, v, o, d_o, lse, heads, scale, *, mask_mode=L.MASK_NONE, text_
              dq=None, dk=None, dv=None):
     """Returns (dq, dk, dv) bf16.  d_o must share o's strides."""
     L.require_cuda(q, k, v, o, d_o, lse, dq, dk, dv, text_time)
-    inner = heads * 64
-    B, nq, nk = _attn_qkv(q, k, v, inner)
-    _attn_rows(o, "o", (B, nq, inner))
-    _attn_rows(d_o, "d_o", (B, nq, inner))
-    if d_o.stride() != o.stride():
-        raise ValueError("d_o must have the same strides as o")
-    _attn_lse(lse, B, heads, nq)
+    B, nq, nk, dq, dk, dv, delta = _attn_bwd_buffers(q, k, v, o, d_o, lse, heads, heads * 64, dq, dk, dv)
     if mask_mode != L.MASK_NONE:
         text_time = _attn_text_time(text_time, B, nq)
-    if dq is None:
-        dq = torch.empty((B, nq, inner), device=q.device, dtype=bf16)
-    if dk is None:
-        dk = torch.empty((B, nk, inner), device=q.device, dtype=bf16)
-    if dv is None:
-        dv = torch.empty((B, nk, inner), device=q.device, dtype=bf16)
-    _attn_rows(dq, "dq", (B, nq, inner))
-    _attn_rows(dk, "dk", (B, nk, inner))
-    _attn_rows(dv, "dv", (B, nk, inner))
-    delta = torch.empty((B, heads, nq), device=q.device, dtype=f32)
-    qb, ldq = _bstride_ld(q, "q")
-    kb, ldk = _bstride_ld(k, "k")
-    vb, ldv = _bstride_ld(v, "v")
-    ob, ldo = _bstride_ld(o, "o")
-    dqb, lddq = _bstride_ld(dq, "dq")
-    dkb, lddk = _bstride_ld(dk, "dk")
-    dvb, lddv = _bstride_ld(dv, "dv")
+    strides = _attn_strides((q, "q"), (k, "k"), (v, "v"), (o, "o"), (dq, "dq"), (dk, "dk"), (dv, "dv"))
     L.check(L.lib().ofk_attn_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), d_o.data_ptr(), lse.data_ptr(),
                                  delta.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, heads, nq, nk,
-                                 qb, ldq, kb, ldk, vb, ldv, ob, ldo, dqb, lddq, dkb, lddk, dvb, lddv, scale, mask_mode,
-                                 L.ptr(text_time), keys_per_media, L.stream_ptr()))
+                                 *strides, scale, mask_mode, L.ptr(text_time), keys_per_media, L.stream_ptr()))
     return dq, dk, dv
 
 
@@ -360,15 +363,11 @@ def attn_dense_fwd(q, k, v, heads, head_dim, scale, *, causal=False, mask=None, 
     L.require_cuda(q, k, v, mask, slopes, pure_causal_flag)
     B, nq, nk = _attn_qkv(q, k, v, heads * head_dim)
     _dense_mask_slopes(mask, slopes, pure_causal_flag, B, heads, nq, nk)
-    out = torch.empty((B, nq, heads * head_dim), device=q.device, dtype=bf16)
-    lse = torch.empty((B, heads, nq), device=q.device, dtype=f32) if want_lse else None
-    qb, ldq = _bstride_ld(q, "q")
-    kb, ldk = _bstride_ld(k, "k")
-    vb, ldv = _bstride_ld(v, "v")
-    ob, ldo = _bstride_ld(out, "out")
+    out, lse = _attn_fwd_outputs(q, B, heads, nq, heads * head_dim, None, want_lse)
+    strides = _attn_strides((q, "q"), (k, "k"), (v, "v"), (out, "out"))
     L.check(L.lib().ofk_attn_dense_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), L.ptr(lse), B, heads,
-                                       head_dim, nq, nk, qb, ldq, kb, ldk, vb, ldv, ob, ldo, scale, int(causal),
-                                       L.ptr(mask), L.ptr(slopes), L.ptr(pure_causal_flag), L.stream_ptr()))
+                                       head_dim, nq, nk, *strides, scale, int(causal), L.ptr(mask), L.ptr(slopes),
+                                       L.ptr(pure_causal_flag), L.stream_ptr()))
     return out, lse
 
 
@@ -502,36 +501,13 @@ def kv_append(src, cache, pos_dev, *, key_mask=None, new_masked=None):
 def attn_dense_bwd(q, k, v, o, d_o, lse, heads, head_dim, scale, *, causal=False, mask=None, slopes=None,
                    pure_causal_flag=None, dq=None, dk=None, dv=None):
     L.require_cuda(q, k, v, o, d_o, lse, mask, slopes, pure_causal_flag, dq, dk, dv)
-    inner = heads * head_dim
-    B, nq, nk = _attn_qkv(q, k, v, inner)
-    _attn_rows(o, "o", (B, nq, inner))
-    _attn_rows(d_o, "d_o", (B, nq, inner))
-    if d_o.stride() != o.stride():
-        raise ValueError("d_o must have the same strides as o")
-    _attn_lse(lse, B, heads, nq)
+    B, nq, nk, dq, dk, dv, delta = _attn_bwd_buffers(q, k, v, o, d_o, lse, heads, heads * head_dim, dq, dk, dv)
     _dense_mask_slopes(mask, slopes, pure_causal_flag, B, heads, nq, nk)
-    if dq is None:
-        dq = torch.empty((B, nq, inner), device=q.device, dtype=bf16)
-    if dk is None:
-        dk = torch.empty((B, nk, inner), device=q.device, dtype=bf16)
-    if dv is None:
-        dv = torch.empty((B, nk, inner), device=q.device, dtype=bf16)
-    _attn_rows(dq, "dq", (B, nq, inner))
-    _attn_rows(dk, "dk", (B, nk, inner))
-    _attn_rows(dv, "dv", (B, nk, inner))
-    delta = torch.empty((B, heads, nq), device=q.device, dtype=f32)
-    qb, ldq = _bstride_ld(q, "q")
-    kb, ldk = _bstride_ld(k, "k")
-    vb, ldv = _bstride_ld(v, "v")
-    ob, ldo = _bstride_ld(o, "o")
-    dqb, lddq = _bstride_ld(dq, "dq")
-    dkb, lddk = _bstride_ld(dk, "dk")
-    dvb, lddv = _bstride_ld(dv, "dv")
+    strides = _attn_strides((q, "q"), (k, "k"), (v, "v"), (o, "o"), (dq, "dq"), (dk, "dk"), (dv, "dv"))
     L.check(L.lib().ofk_attn_dense_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), d_o.data_ptr(),
                                        lse.data_ptr(), delta.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
-                                       B, heads, head_dim, nq, nk, qb, ldq, kb, ldk, vb, ldv, ob, ldo, dqb, lddq, dkb,
-                                       lddk, dvb, lddv, scale, int(causal), L.ptr(mask), L.ptr(slopes),
-                                       L.ptr(pure_causal_flag), L.stream_ptr()))
+                                       B, heads, head_dim, nq, nk, *strides, scale, int(causal), L.ptr(mask),
+                                       L.ptr(slopes), L.ptr(pure_causal_flag), L.stream_ptr()))
     return dq, dk, dv
 
 
