@@ -96,8 +96,10 @@ int ofk_gemm_bf16_grouped(int epi, int a_mn_major, int b_mn_major, const void* A
  *   x: [rows, D] f32 (ldx).  y: bf16 (y_is_f32 = 0) or f32, written at
  *   row index  (r / rows_per_group) * group_stride + group_offset + r % rows_per_group  of y (ldy) --
  *   this lets two LayerNorms write the two halves of PerceiverAttention's cat((x, latents), -2)
- *   (helpers.py:53) in place (rows_per_group <= 0: identity mapping).  mean/rstd: [rows] f32 outputs (may be
- *   NULL).  D % 4 == 0, D <= 4096.
+ *   (helpers.py:53) in place (rows_per_group <= 0: identity mapping; otherwise 0 <= group_offset and
+ *   group_offset + rows_per_group <= group_stride, OFK_ERR_ARG).  mean/rstd: [rows] f32 outputs (may be NULL).
+ *   D % 4 == 0, D <= 4096.  ldx, ldy multiples of 4; x, gamma, beta and an f32 y 16-byte aligned, a bf16 y 8-byte
+ *   aligned (OFK_ERR_ALIGN).  Every argument is checked before the first CUDA call.
  */
 int ofk_layernorm_fwd(const float* x, long long ldx, const float* gamma, const float* beta,
                       float eps, int rows, int D, void* y, int y_is_f32, long long ldy, int rows_per_group,
@@ -106,7 +108,9 @@ int ofk_layernorm_fwd(const float* x, long long ldx, const float* gamma, const f
 /* LayerNorm backward.  dy: [rows, D] bf16 or f32 (same row mapping as fwd via dy_* group args);
  * x: f32 [rows, D]; dx(f32) = LN'(dy) (+ dx_add if non-NULL; dx_add may alias dx); dx NULL = parameter
  * gradients only (PerceiverAttention.norm_media: its input, the frozen ViT features, needs no gradient).
- * dgamma/dbeta (f32 [D]) are ACCUMULATED (+=).  workspace: >= ofk_layernorm_bwd_workspace(rows, D) bytes. */
+ * dgamma/dbeta (f32 [D]) are ACCUMULATED (+=).  workspace: >= ofk_layernorm_bwd_workspace(rows, D) bytes.
+ * Requirements: the group mapping, D and strides as in the forward; x, gamma, dx, dx_add, workspace and an f32 dy
+ * 16-byte aligned, a bf16 dy 8-byte aligned (OFK_ERR_ALIGN), all checked before the first CUDA call. */
 long long ofk_layernorm_bwd_workspace(int rows, int D);
 int ofk_layernorm_bwd(const void* dy, int dy_is_f32, long long lddy, int rows_per_group, int group_stride,
                       int group_offset, const float* x, long long ldx, const float* gamma, const float* mean,
@@ -251,7 +255,8 @@ long long ofk_reduce_workspace_bytes(void);
 /* Gate backward (autograd of helpers.py:274,277):
  *   dbranch(bf16)[i] = dout(f32)[i] * tanh(*gate);  dgate[0] += (1 - tanh(*gate)^2) * sum_i dout[i]*branch(bf16)[i]
  * gate NULL => multiplier 1 and no dgate (plain residual branch, helpers.py:130-131).  workspace: see above (may be
- * NULL when no dgate is wanted). */
+ * NULL when no dgate is wanted).  n % 8 == 0 (OFK_ERR_ARG); dout, dbranch and (with a gate) branch 16-byte aligned
+ * (OFK_ERR_ALIGN). */
 int ofk_gate_bwd(const float* dout, const void* branch, const float* gate, void* dbranch, float* dgate,
                  long long n, float* workspace, void* stream);
 
@@ -263,7 +268,9 @@ int ofk_add_f32(float* dst, const float* src, long long n, void* stream);
  * stride-P conv of open_clip VisionTransformer.conv1 (third party; call site flamingo.py:195). */
 int ofk_patchify(const float* images, int n, int H, int W, int P, void* patches, long long ldp, void* stream);
 
-/* tokens[n, 1 + g, D] f32 = cat(class_emb, patch_emb(bf16)[n, g, D]) + pos_emb[1+g, D]   (open_clip ViT) */
+/* tokens[n, 1 + g, D] f32 = cat(class_emb, patch_emb(bf16)[n, g, D]) + pos_emb[1+g, D]   (open_clip ViT)
+ * g >= 0, D > 0 and D % 4 == 0 (OFK_ERR_ARG); patch_emb may be NULL when g == 0; patch_emb 8-byte aligned, class_emb, pos_emb, tokens 16-byte aligned
+ * (OFK_ERR_ALIGN). */
 int ofk_vit_assemble(const void* patch_emb, const float* class_emb, const float* pos_emb, int n, int g, int D,
                      float* tokens, void* stream);
 
@@ -271,7 +278,10 @@ int ofk_vit_assemble(const void* patch_emb, const float* class_emb, const float*
  * flamingo.py:111-117 -> HF ForCausalLMLoss: float logits, labels shifted by one, mean over non-ignored).
  *   logits: [rows = B*T, vocab] bf16 or f32 (ld); labels: [B, T] int64 (host-unshifted when shift_labels = 1).
  *   fwd: lse[rows]; *loss_sum += sum(lse - logit[target]); *count += #non-ignored rows.  (caller zeroes them)
- *   bwd: dlogits = (softmax - onehot) * (*grad_scale) / max(*count, 1) for non-ignored rows, 0 otherwise. */
+ *   bwd: dlogits = (softmax - onehot) * (*grad_scale) / max(*count, 1) for non-ignored rows, 0 otherwise.
+ *   Targets outside [0, vocab) count as ignored.  bf16 rows are read 8 at a time when vocab, ld (and ldd) are
+ *   multiples of 8 and logits (and dlogits) are 16-byte aligned, one at a time otherwise.
+ *   Logits may be -inf (masked vocabulary entries). */
 int ofk_ce_fwd(const void* logits, int logits_is_f32, long long ld, long long rows, int vocab,
                const long long* labels, int T, int shift_labels, long long ignore_index, float* lse,
                float* loss_sum, float* count, void* stream);

@@ -249,6 +249,8 @@ __global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ x,
 
 using namespace ofk;
 
+static bool misaligned(const void* p, unsigned bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) != 0; }
+
 extern "C" int ofk_text_time(const long long* input_ids, long long media_token_id, int batch, int t_txt, int n_loc,
                              const unsigned char* media_locations, int use_cached_media, int* text_time, void* stream) {
   if (!text_time || (!input_ids && !media_locations)) return ofk_set_error(OFK_ERR_ARG, "text_time: null pointer");
@@ -293,6 +295,8 @@ extern "C" int ofk_gate_bwd(const float* dout, const void* branch, const float* 
   if (want_dgate && !workspace) return ofk_set_error(OFK_ERR_ARG, "gate_bwd: dgate needs the reduction workspace");
   if (n <= 0) return 0;
   if (n % 8 != 0) return ofk_set_error(OFK_ERR_ARG, "gate_bwd: n must be a multiple of 8");
+  if (misaligned(dout, 16) || misaligned(dbranch, 16) || (gate && misaligned(branch, 16)))
+    return ofk_set_error(OFK_ERR_ALIGN, "gate_bwd: dout, branch and dbranch must be 16-byte aligned");
   const int grid = grid_for(n / 8, 256);
   gate_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(dout, (const __nv_bfloat16*)branch, gate, (__nv_bfloat16*)dbranch,
                                                           want_dgate ? workspace : nullptr, n);
@@ -330,9 +334,12 @@ extern "C" int ofk_patchify(const float* images, int n, int H, int W, int P, voi
 
 extern "C" int ofk_vit_assemble(const void* patch_emb, const float* class_emb, const float* pos_emb, int n, int g, int D,
                                 float* tokens, void* stream) {
-  if (!patch_emb || !class_emb || !pos_emb || !tokens) return ofk_set_error(OFK_ERR_ARG, "vit_assemble: null pointer");
+  if ((g != 0 && !patch_emb) || !class_emb || !pos_emb || !tokens)   // g == 0: class tokens only, no patch is read
+    return ofk_set_error(OFK_ERR_ARG, "vit_assemble: null pointer");
   if (n <= 0) return 0;
-  if (D % 4 != 0) return ofk_set_error(OFK_ERR_ARG, "vit_assemble: D must be a multiple of 4");
+  if (g < 0 || D <= 0 || D % 4 != 0) return ofk_set_error(OFK_ERR_ARG, "vit_assemble: g >= 0 and D > 0 a multiple of 4");
+  if (misaligned(patch_emb, 8) || misaligned(class_emb, 16) || misaligned(pos_emb, 16) || misaligned(tokens, 16))
+    return ofk_set_error(OFK_ERR_ALIGN, "vit_assemble: patch_emb must be 8-byte aligned, class_emb, pos_emb, tokens 16");
   vit_assemble_kernel<<<grid_for((long long)n * (g + 1) * (D / 4), 256), 256, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)patch_emb, class_emb, pos_emb, n, g, D, tokens);
   OFK_CHECK_LAUNCH();

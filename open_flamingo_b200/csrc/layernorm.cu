@@ -185,6 +185,14 @@ __global__ void __launch_bounds__(256) ln_bwd_reduce_kernel(const float* __restr
   }
 }
 
+static bool misaligned(const void* p, unsigned bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) != 0; }
+
+// The grouped row mapping writes group g's rows to [g * group_stride + group_offset, ... + rows_per_group): the groups
+// must not overlap one another.
+static bool bad_group_map(int rows_per_group, int group_stride, int group_offset) {
+  return rows_per_group > 0 && (group_offset < 0 || (long long)group_offset + rows_per_group > group_stride);
+}
+
 }  // namespace ofk
 
 extern "C" int ofk_layernorm_fwd(const float* x, long long ldx, const float* gamma, const float* beta, float eps,
@@ -194,7 +202,11 @@ extern "C" int ofk_layernorm_fwd(const float* x, long long ldx, const float* gam
   if (!x || !gamma || !beta || !y) return ofk_set_error(OFK_ERR_ARG, "layernorm: null pointer");
   if (rows <= 0) return 0;
   if (D <= 0 || D % 4 != 0 || D > 4096) return ofk_set_error(OFK_ERR_ARG, "layernorm: D must be a multiple of 4, <= 4096");
+  if (bad_group_map(rows_per_group, group_stride, group_offset))
+    return ofk_set_error(OFK_ERR_ARG, "layernorm: group_offset + rows_per_group exceeds group_stride");
   if (ldx % 4 != 0 || ldy % 4 != 0) return ofk_set_error(OFK_ERR_ALIGN, "layernorm: row strides must be multiples of 4");
+  if (misaligned(x, 16) || misaligned(gamma, 16) || misaligned(beta, 16) || misaligned(y, y_is_f32 ? 16 : 8))
+    return ofk_set_error(OFK_ERR_ALIGN, "layernorm: x, gamma, beta and an f32 y must be 16-byte aligned, a bf16 y 8-byte");
   cudaStream_t s = (cudaStream_t)stream_;
   const int grid = (rows + 3) / 4;
   if (D <= 1024)
@@ -223,6 +235,12 @@ extern "C" int ofk_layernorm_bwd(const void* dy, int dy_is_f32, long long lddy, 
   if (D <= 0 || D % 4 != 0 || D > 4096) return ofk_set_error(OFK_ERR_ARG, "layernorm bwd: D must be a multiple of 4, <= 4096");
   if (ldx % 4 != 0 || lddy % 4 != 0 || lddx % 4 != 0 || (dx_add && ldadd % 4 != 0))
     return ofk_set_error(OFK_ERR_ALIGN, "layernorm bwd: row strides must be multiples of 4");
+  if (bad_group_map(rows_per_group, group_stride, group_offset))
+    return ofk_set_error(OFK_ERR_ARG, "layernorm bwd: group_offset + rows_per_group exceeds group_stride");
+  if (misaligned(dy, dy_is_f32 ? 16 : 8) || misaligned(x, 16) || misaligned(gamma, 16) || misaligned(dx, 16) ||
+      misaligned(dx_add, 16) || misaligned(workspace, 16))
+    return ofk_set_error(OFK_ERR_ALIGN, "layernorm bwd: x, gamma, dx, dx_add, workspace and an f32 dy must be 16-byte "
+                                        "aligned, a bf16 dy 8-byte");
   cudaStream_t s = (cudaStream_t)stream_;
   const int nblocks = rows < LNB_MAX_BLOCKS ? rows : LNB_MAX_BLOCKS;
   float* part = (dgamma || dbeta) ? reinterpret_cast<float*>(workspace) : nullptr;

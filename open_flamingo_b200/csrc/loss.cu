@@ -25,12 +25,14 @@ __device__ __forceinline__ long long row_target(const long long* labels, int T, 
 }
 
 // lse[row] (natural log) of every row.
-__global__ void __launch_bounds__(256) ce_fwd_kernel(const void* __restrict__ logits, int is_f32, long long ld, int V,
-                                                     float* __restrict__ lse) {
+// vec: the rows may be read 8 bf16 at a time (see vec8_rows).
+__global__ void __launch_bounds__(256) ce_fwd_kernel(const void* __restrict__ logits, int is_f32, int vec, long long ld,
+                                                     int V, float* __restrict__ lse) {
   __shared__ float s_m[8], s_l[8];
   const long long row = blockIdx.x;
   float m = -INFINITY, l = 0.f;
-  if (!is_f32 && (V % 8 == 0) && (ld % 8 == 0)) {
+  // The running max is subtracted as 0 while it is still -inf (every logit so far was -inf): -inf - -inf would be NaN.
+  if (vec) {
     const uint4* p = reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(logits) + row * ld);
     for (int i = threadIdx.x; i < V / 8; i += 256) {
       const uint4 u = p[i];
@@ -38,17 +40,19 @@ __global__ void __launch_bounds__(256) ce_fwd_kernel(const void* __restrict__ lo
       float mx = m;
 #pragma unroll
       for (int j = 0; j < 8; ++j) mx = fmaxf(mx, v[j]);
+      const float ms = mx == -INFINITY ? 0.f : mx;
       float acc = 0.f;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) acc += __expf(v[j] - mx);
-      l = l * __expf(m - mx) + acc;
+      for (int j = 0; j < 8; ++j) acc += __expf(v[j] - ms);
+      l = l * __expf(m - ms) + acc;
       m = mx;
     }
   } else {
     for (int i = threadIdx.x; i < V; i += 256) {
       const float v = load_logit(logits, is_f32, row * ld + i);
       const float mx = fmaxf(m, v);
-      l = l * __expf(m - mx) + __expf(v - mx);
+      const float ms = mx == -INFINITY ? 0.f : mx;
+      l = l * __expf(m - ms) + __expf(v - ms);
       m = mx;
     }
   }
@@ -99,7 +103,7 @@ __global__ void __launch_bounds__(256) ce_sum_kernel(const void* __restrict__ lo
 }
 
 // dlogits[row, v] = (softmax(row)[v] - [v == target]) * (*gscale) / (*count) for non-ignored rows, else 0.
-__global__ void __launch_bounds__(256) ce_bwd_kernel(const void* __restrict__ logits, int is_f32, long long ld, int V,
+__global__ void __launch_bounds__(256) ce_bwd_kernel(const void* __restrict__ logits, int is_f32, int vec, long long ld, int V,
                                                      const long long* __restrict__ labels, int T, int shift,
                                                      long long ignore_index, const float* __restrict__ lse,
                                                      const float* __restrict__ gscale, const float* __restrict__ count,
@@ -109,7 +113,7 @@ __global__ void __launch_bounds__(256) ce_bwd_kernel(const void* __restrict__ lo
   const bool valid = tgt != ignore_index && tgt >= 0 && tgt < V;
   const float sc = valid ? __ldg(gscale) / fmaxf(__ldg(count), 1.0f) : 0.f;
   const float L = lse[row];
-  if (!is_f32 && (V % 8 == 0) && (ld % 8 == 0) && (ldd % 8 == 0)) {
+  if (vec) {
     const uint4* p = reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(logits) + row * ld);
     uint4* d = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(dlogits) + row * ldd);
     for (int i = threadIdx.x; i < V / 8; i += 256) {
@@ -132,6 +136,12 @@ __global__ void __launch_bounds__(256) ce_bwd_kernel(const void* __restrict__ lo
   }
 }
 
+// The 8-wide bf16 path reads (and writes) each row as uint4: it needs every row start 16-byte aligned.  Any other
+// layout takes the scalar path, which is correct for every pointer and stride.
+static int vec8_rows(const void* p, int is_f32, long long ld, int V) {
+  return !is_f32 && V % 8 == 0 && ld % 8 == 0 && (reinterpret_cast<uintptr_t>(p) & 15) == 0;
+}
+
 }  // namespace ofk
 
 extern "C" int ofk_ce_fwd(const void* logits, int logits_is_f32, long long ld, long long rows, int vocab,
@@ -140,7 +150,8 @@ extern "C" int ofk_ce_fwd(const void* logits, int logits_is_f32, long long ld, l
   if (!logits || !labels || !lse || !loss_sum || !count) return ofk_set_error(OFK_ERR_ARG, "ce_fwd: null pointer");
   if (rows <= 0) return 0;
   if (vocab <= 0 || T <= 0 || rows % T != 0) return ofk_set_error(OFK_ERR_ARG, "ce_fwd: rows must be a multiple of T");
-  ofk::ce_fwd_kernel<<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(logits, logits_is_f32, ld, vocab, lse);
+  const int vec = ofk::vec8_rows(logits, logits_is_f32, ld, vocab);
+  ofk::ce_fwd_kernel<<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(logits, logits_is_f32, vec, ld, vocab, lse);
   OFK_CHECK_LAUNCH();
   ofk::ce_sum_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(logits, logits_is_f32, ld, rows, vocab, labels, T, shift_labels,
                                                           ignore_index, lse, loss_sum, count);
@@ -154,8 +165,10 @@ extern "C" int ofk_ce_bwd(const void* logits, int logits_is_f32, long long ld, l
   if (!logits || !labels || !lse || !grad_scale || !count || !dlogits) return ofk_set_error(OFK_ERR_ARG, "ce_bwd: null pointer");
   if (rows <= 0) return 0;
   if (vocab <= 0 || T <= 0 || rows % T != 0) return ofk_set_error(OFK_ERR_ARG, "ce_bwd: rows must be a multiple of T");
-  ofk::ce_bwd_kernel<<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(logits, logits_is_f32, ld, vocab, labels, T, shift_labels,
-                                                                        ignore_index, lse, grad_scale, count, dlogits, ldd);
+  const int vec = ofk::vec8_rows(logits, logits_is_f32, ld, vocab) && ofk::vec8_rows(dlogits, logits_is_f32, ldd, vocab);
+  ofk::ce_bwd_kernel<<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(logits, logits_is_f32, vec, ld, vocab, labels, T,
+                                                                        shift_labels, ignore_index, lse, grad_scale, count,
+                                                                        dlogits, ldd);
   OFK_CHECK_LAUNCH();
   return 0;
 }

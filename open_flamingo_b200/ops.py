@@ -19,6 +19,32 @@ def _rowmajor_2d(t, name):
         raise ValueError(f"{name} must be 2-D with unit inner stride, got shape {tuple(t.shape)} stride {t.stride()}")
 
 
+def _vector(t, name, dtype, n, at_least=False):
+    """t: a contiguous `dtype` tensor of exactly n elements (at least n with at_least)."""
+    if t.dtype != dtype or not t.is_contiguous() or (t.numel() < n if at_least else t.numel() != n):
+        raise ValueError(f"{name} must be a contiguous {dtype} tensor of {'>= ' if at_least else ''}{n} elements, got "
+                         f"{tuple(t.shape)} {t.dtype} stride {t.stride()}")
+
+
+def _rows2d(t, name, dtypes, rows, D):
+    """t: 2-D, unit inner stride, one of `dtypes`, at least `rows` rows of at least D columns."""
+    _rowmajor_2d(t, name)
+    if t.dtype not in dtypes or t.shape[0] < rows or t.shape[1] < D:
+        raise ValueError(f"{name} must be a {' or '.join(map(str, dtypes))} tensor of >= {rows} rows and >= {D} columns, "
+                         f"got {tuple(t.shape)} {t.dtype}")
+
+
+def _mapped_rows(rows, rows_per_group, group_stride, group_offset):
+    """Rows of the buffer the LayerNorm group mapping reaches (row r -> (r // rpg) * stride + offset + r % rpg)."""
+    if rows_per_group <= 0:
+        return rows
+    if group_offset < 0 or group_offset + rows_per_group > group_stride:
+        raise ValueError(f"layernorm group mapping: need 0 <= group_offset and group_offset + rows_per_group <= "
+                         f"group_stride, got ({rows_per_group}, {group_stride}, {group_offset})")
+    last = rows - 1
+    return (last // rows_per_group) * group_stride + group_offset + last % rows_per_group + 1
+
+
 _comm_in_flight = False
 # SMs every persistent GEMM grid leaves to NCCL while gradient-chunk all-reduces are in flight (world > 1 only; 0 = none).
 # A persistent grid that owns every SM lets the all-reduce kernels in only at GEMM boundaries, so the "overlapped" reduction
@@ -94,9 +120,12 @@ def layernorm_fwd(x, gamma, beta, eps=1e-5, *, out=None, out_f32=False, rows_per
     if x.dtype != f32:
         raise ValueError("layernorm input must be float32 (the residual stream is fp32)")
     rows, D = x.shape
+    L.require_cuda(gamma, beta, out)
+    _vector(gamma, "gamma", f32, D)
+    _vector(beta, "beta", f32, D)
     if out is None:
         out = torch.empty((rows, D), device=x.device, dtype=f32 if out_f32 else bf16)
-    _rowmajor_2d(out, "out")
+    _rows2d(out, "out", (f32, bf16), _mapped_rows(rows, rows_per_group, group_stride, group_offset), D)
     y_is_f32 = out.dtype == f32
     mean = torch.empty(rows, device=x.device, dtype=f32) if want_stats else None
     rstd = torch.empty(rows, device=x.device, dtype=f32) if want_stats else None
@@ -123,10 +152,21 @@ def layernorm_bwd(dy, x, gamma, mean, rstd, *, dgamma=None, dbeta=None, dx=None,
                   group_stride=0, group_offset=0, want_dx=True):
     """dx = LN'(dy) (+ dx_add); dgamma/dbeta are accumulated in place.  dy may be bf16 or f32 (mapped rows).
     want_dx=False: only the affine-parameter gradients are produced."""
-    L.require_cuda(dy, x)
-    _rowmajor_2d(dy, "dy")
+    L.require_cuda(dy, x, gamma, mean, rstd, dgamma, dbeta, dx, dx_add)
     _rowmajor_2d(x, "x")
+    if x.dtype != f32:
+        raise ValueError("layernorm input must be float32 (the residual stream is fp32)")
     rows, D = x.shape
+    _rows2d(dy, "dy", (f32, bf16), _mapped_rows(rows, rows_per_group, group_stride, group_offset), D)
+    _vector(gamma, "gamma", f32, D)
+    _vector(mean, "mean", f32, rows)
+    _vector(rstd, "rstd", f32, rows)
+    for t, name in ((dgamma, "dgamma"), (dbeta, "dbeta")):
+        if t is not None:
+            _vector(t, name, f32, D)
+    for t, name in ((dx, "dx"), (dx_add, "dx_add")):
+        if t is not None:
+            _rows2d(t, name, (f32,), rows, D)
     if dx is None and want_dx:
         dx = torch.empty((rows, D), device=x.device, dtype=f32)
     ws = _ln_workspace(x.device, rows, D)
@@ -284,10 +324,13 @@ def text_time(input_ids=None, media_token_id=0, media_locations=None, use_cached
 
 
 def cast_bf16(src, out=None):
-    L.require_cuda(src)
+    L.require_cuda(src, out)
+    if src.dtype != f32:
+        raise ValueError("cast_bf16 source must be float32")
     src = src.contiguous()
     if out is None:
         out = torch.empty(src.shape, device=src.device, dtype=bf16)
+    _vector(out, "out", bf16, src.numel())
     L.check(L.lib().ofk_cast_f32_bf16(src.data_ptr(), out.data_ptr(), src.numel(), L.stream_ptr()))
     return out
 
@@ -307,9 +350,15 @@ def _reduce_workspace(device):
 
 def gate_bwd(dout, branch, gate, dgate):
     """dbranch(bf16) = dout * tanh(gate); dgate += (1 - tanh^2) * <dout, branch>.  gate None: plain cast."""
-    L.require_cuda(dout)
-    if not dout.is_contiguous() or (branch is not None and not branch.is_contiguous()):
-        raise ValueError("gate_bwd operands must be contiguous")
+    L.require_cuda(dout, branch, gate, dgate)
+    _vector(dout, "dout", f32, dout.numel())
+    if gate is not None:
+        _vector(gate, "gate", f32, 1)
+        if branch is None:
+            raise ValueError("gate_bwd with a gate needs the branch")
+        _vector(branch, "branch", bf16, dout.numel())
+    if dgate is not None:
+        _vector(dgate, "dgate", f32, 1)
     dbranch = torch.empty(dout.shape, device=dout.device, dtype=bf16)
     ws = _reduce_workspace(dout.device) if (gate is not None and dgate is not None) else None
     L.check(L.lib().ofk_gate_bwd(dout.data_ptr(), L.ptr(branch), L.ptr(gate), dbranch.data_ptr(), L.ptr(dgate),
@@ -318,6 +367,10 @@ def gate_bwd(dout, branch, gate, dgate):
 
 
 def add_(dst, src):
+    """dst += src, both contiguous float32 of the same size."""
+    L.require_cuda(dst, src)
+    _vector(dst, "dst", f32, dst.numel())
+    _vector(src, "src", f32, dst.numel())
     L.check(L.lib().ofk_add_f32(dst.data_ptr(), src.data_ptr(), dst.numel(), L.stream_ptr()))
     return dst
 
@@ -325,6 +378,8 @@ def add_(dst, src):
 def patchify(images, patch, ldp):
     """images [n,3,H,W] f32 -> [n*g, ldp] bf16 patch rows (conv-weight column order), zero padded."""
     L.require_cuda(images)
+    if images.dtype != f32 or images.dim() != 4 or images.shape[1] != 3:
+        raise ValueError(f"images must be float32 [n, 3, H, W], got {tuple(images.shape)} {images.dtype}")
     images = images.contiguous()
     n, _, H, W = images.shape
     g = (H // patch) * (W // patch)
@@ -334,6 +389,16 @@ def patchify(images, patch, ldp):
 
 
 def vit_assemble(patch_emb, class_emb, pos_emb, n, g, D):
+    """patch_emb: contiguous bf16 [n*g, D]; class_emb: f32 [D]; pos_emb: contiguous f32 [g+1, D].  Returns f32
+    [n*(g+1), D] tokens."""
+    L.require_cuda(patch_emb, class_emb, pos_emb)
+    if patch_emb.dtype != bf16 or tuple(patch_emb.shape) != (n * g, D) or not patch_emb.is_contiguous():
+        raise ValueError(f"patch_emb must be a contiguous bf16 [{n * g}, {D}] tensor, got {tuple(patch_emb.shape)} "
+                         f"{patch_emb.dtype}")
+    _vector(class_emb, "class_emb", f32, D)
+    if pos_emb.dtype != f32 or tuple(pos_emb.shape) != (g + 1, D) or not pos_emb.is_contiguous():
+        raise ValueError(f"pos_emb must be a contiguous float32 [{g + 1}, {D}] tensor, got {tuple(pos_emb.shape)} "
+                         f"{pos_emb.dtype}")
     tok = torch.empty((n * (g + 1), D), device=patch_emb.device, dtype=f32)
     L.check(L.lib().ofk_vit_assemble(patch_emb.data_ptr(), class_emb.data_ptr(), pos_emb.data_ptr(), n, g, D,
                                      tok.data_ptr(), L.stream_ptr()))
@@ -342,7 +407,18 @@ def vit_assemble(patch_emb, class_emb, pos_emb, n, g, D):
 
 def adamw_(param, grad, exp_avg, exp_avg_sq, w_bf16, lr, beta1, beta2, eps, wd, step, clip_scale=None, step_dev=None,
            lr_dev=None):
-    """step: host int (ignored when step_dev, a device float tensor holding the step count, is given)."""
+    """step: host int (ignored when step_dev, a device float tensor holding the step count, is given).
+    param, grad, exp_avg, exp_avg_sq: contiguous float32 of one size; w_bf16: contiguous bf16 of that size or None;
+    clip_scale, step_dev, lr_dev: float32 device scalars or None."""
+    L.require_cuda(param, grad, exp_avg, exp_avg_sq, w_bf16, clip_scale, step_dev, lr_dev)
+    n = param.numel()
+    for t, name in ((param, "param"), (grad, "grad"), (exp_avg, "exp_avg"), (exp_avg_sq, "exp_avg_sq")):
+        _vector(t, name, f32, n)
+    if w_bf16 is not None:
+        _vector(w_bf16, "w_bf16", bf16, n)
+    for t, name in ((clip_scale, "clip_scale"), (step_dev, "step_dev"), (lr_dev, "lr_dev")):
+        if t is not None:
+            _vector(t, name, f32, 1, at_least=True)
     bc1 = 1.0 - beta1 ** max(step, 1)
     bc2 = 1.0 - beta2 ** max(step, 1)
     L.check(L.lib().ofk_adamw(param.data_ptr(), grad.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(),
@@ -351,6 +427,10 @@ def adamw_(param, grad, exp_avg, exp_avg_sq, w_bf16, lr, beta1, beta2, eps, wd, 
 
 
 def sumsq_(x, out):
+    """out[0] += sum(x * x); x contiguous float32, out a float32 device scalar."""
+    L.require_cuda(x, out)
+    _vector(x, "x", f32, x.numel())
+    _vector(out, "out", f32, 1, at_least=True)
     L.check(L.lib().ofk_sumsq(x.data_ptr(), x.numel(), out.data_ptr(), _reduce_workspace(x.device).data_ptr(),
                               L.stream_ptr()))
     return out

@@ -140,51 +140,6 @@ def test_gemm_errors(ops, L):
         ops.gemm(a, a, epi=L.EPI_BIAS_BF16)  # missing bias
 
 
-# ------------------------------------------------------------------ LayerNorm
-@pytest.mark.parametrize("rows,D", [(37, 64), (513, 1024), (300, 2048), (129, 4096)])
-def test_layernorm_fwd_bwd(ops, rows, D):
-    torch.manual_seed(3)
-    x = (torch.randn(rows, D, device="cuda") * 2 + 0.5)
-    g = torch.randn(D, device="cuda")
-    b = torch.randn(D, device="cuda")
-    xr = x.clone().requires_grad_(True)
-    gr = g.clone().requires_grad_(True)
-    brr = b.clone().requires_grad_(True)
-    ref = torch.nn.functional.layer_norm(xr, (D,), gr, brr, 1e-5)
-    y32, mean, rstd = ops.layernorm_fwd(x, g, b, out_f32=True)
-    close(y32, ref, 2e-5, "ln fwd f32")
-    y16, _, _ = ops.layernorm_fwd(x, g, b)
-    close(y16, ref.to(bf16), 1e-2, "ln fwd bf16")
-    dy = torch.randn(rows, D, device="cuda")
-    ref.backward(dy)
-    dg = torch.zeros(D, device="cuda")
-    db = torch.zeros(D, device="cuda")
-    add = torch.randn(rows, D, device="cuda")
-    dx = ops.layernorm_bwd(dy, x, g, mean, rstd, dgamma=dg, dbeta=db, dx_add=add)
-    close(dx - add, xr.grad, 1e-4, "ln dx")
-    close(dg, gr.grad, 1e-4, "ln dgamma")
-    close(db, brr.grad, 1e-4, "ln dbeta")
-    # bf16 dy path
-    dx2 = ops.layernorm_bwd(dy.to(bf16), x, g, mean, rstd)
-    close(dx2, xr.grad, 2e-2, "ln dx (bf16 dy)")
-
-
-def test_layernorm_group_mapping(ops):
-    """Two LayerNorms fill the halves of cat((x, latents), -2) in place (helpers.py:47-53)."""
-    torch.manual_seed(4)
-    U, v, n, D = 3, 20, 8, 128
-    x = torch.randn(U * v, D, device="cuda")
-    lat = torch.randn(U * n, D, device="cuda")
-    g1, b1 = torch.randn(D, device="cuda"), torch.randn(D, device="cuda")
-    g2, b2 = torch.randn(D, device="cuda"), torch.randn(D, device="cuda")
-    buf = torch.zeros(U * (v + n), D, device="cuda", dtype=bf16)
-    ops.layernorm_fwd(x, g1, b1, out=buf, rows_per_group=v, group_stride=v + n, group_offset=0)
-    ops.layernorm_fwd(lat, g2, b2, out=buf, rows_per_group=n, group_stride=v + n, group_offset=v)
-    ref = torch.cat([torch.nn.functional.layer_norm(x, (D,), g1, b1).view(U, v, D),
-                     torch.nn.functional.layer_norm(lat, (D,), g2, b2).view(U, n, D)], dim=1).reshape(-1, D)
-    close(buf, ref.to(bf16), 1e-2, "ln concat mapping")
-
-
 # ------------------------------------------------------------------ attention
 def ref_attention(q, k, v, heads, scale, mask_mode, tt, kpm):
     """Plain fp32 restatement (per helpers.py:190-232 semantics) on bf16-rounded inputs."""
@@ -298,69 +253,6 @@ def test_text_time(ops):
     assert torch.equal(ops.text_time(media_locations=loc), ref)
     cached = ops.text_time(media_locations=loc, use_cached_media=True, t_txt=3)
     assert torch.equal(cached, loc.sum(-1, keepdim=True).int().expand(-1, 3))
-
-
-def test_gate_bwd_cast_add(ops):
-    torch.manual_seed(9)
-    n = 8 * 1000
-    dout = torch.randn(n, device="cuda")
-    branch = torch.randn(n, device="cuda").to(bf16)
-    gate = torch.tensor([0.3], device="cuda")
-    dgate = torch.zeros(1, device="cuda")
-    dbr = ops.gate_bwd(dout, branch, gate, dgate)
-    t = math.tanh(0.3)
-    close(dbr, (dout * t).to(bf16), 1e-2, "dbranch")
-    close(dgate, ((1 - t * t) * (dout * branch.float()).sum()).view(1), 1e-4, "dgate")
-    close(ops.gate_bwd(dout, None, None, None), dout.to(bf16), 1e-2, "plain cast branch")
-    x = torch.randn(1003, device="cuda")
-    close(ops.cast_bf16(x), x.to(bf16), 0, "cast")
-    y = torch.randn(1003, device="cuda")
-    ref = x + y
-    close(ops.add_(x, y), ref, 0, "add")
-
-
-def test_patchify_assemble(ops):
-    torch.manual_seed(10)
-    n, H, P, D = 2, 28, 14, 64
-    img = torch.randn(n, 3, H, H, device="cuda")
-    ldp = 640
-    pt = ops.patchify(img, P, ldp)
-    w = torch.randn(D, 3, P, P, device="cuda")
-    ref = torch.nn.functional.conv2d(img.to(bf16).float(), w.to(bf16).float(), stride=P)  # [n, D, 2, 2]
-    ref = ref.flatten(2).transpose(1, 2).reshape(-1, D)
-    wp = torch.zeros(D, ldp, device="cuda", dtype=bf16)
-    wp[:, :3 * P * P] = w.reshape(D, -1).to(bf16)
-    got = pt.float() @ wp.float().t()
-    close(got, ref, 1e-4, "patchify == strided conv")
-    assert pt[:, 3 * P * P:].abs().max().item() == 0
-    g = (H // P) ** 2
-    pe = torch.randn(n * g, D, device="cuda").to(bf16)
-    cls = torch.randn(D, device="cuda")
-    pos = torch.randn(g + 1, D, device="cuda")
-    tok = ops.vit_assemble(pe, cls, pos, n, g, D).view(n, g + 1, D)
-    ref = torch.cat([cls.expand(n, 1, D), pe.float().view(n, g, D)], 1) + pos
-    close(tok, ref, 1e-6, "vit assemble")
-
-
-def test_adamw_sumsq(ops):
-    torch.manual_seed(11)
-    n = 10007
-    p = torch.randn(n, device="cuda")
-    g = torch.randn(n, device="cuda")
-    pr = p.clone().requires_grad_(True)
-    opt = torch.optim.AdamW([pr], lr=1e-2, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.1)
-    m = torch.zeros(n, device="cuda")
-    v = torch.zeros(n, device="cuda")
-    w16 = torch.empty(n, device="cuda", dtype=bf16)
-    for step in (1, 2, 3):
-        pr.grad = g.clone()
-        opt.step()
-        ops.adamw_(p, g, m, v, w16, 1e-2, 0.9, 0.999, 1e-8, 0.1, step)
-    close(p, pr.detach(), 1e-5, "adamw")
-    close(w16, p.to(bf16), 0, "adamw bf16 copy")
-    out = torch.zeros(1, device="cuda")
-    ops.sumsq_(g, out)
-    close(out, (g * g).sum().view(1), 1e-5, "sumsq")
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
