@@ -181,8 +181,9 @@ int ofk_attn_dense_bwd(const void* q, const void* k, const void* v, const void* 
                        long long dv_bstride, long long lddv, float scale, int causal, const unsigned char* mask,
                        const float* slopes, const int* pure_causal_flag, void* stream);
 
-/* Decode attention of the same blocks with a KV cache (HF MptAttention with past_key_values, one new token): split-KV
- * ("flash-decoding") over the cache, csrc/attention_decode.cu.  Semantics are those of ofk_attn_dense_fwd at nq = 1:
+/* Decode attention of the same blocks with a KV cache (HF MptAttention or GPTNeoXAttention with past_key_values, one new
+ * token): split-KV ("flash-decoding") over the cache, csrc/attention_decode.cu.  Semantics are those of
+ * ofk_attn_dense_fwd at nq = 1:
  *   S = scale * q K^T + slopes[h] * key_index  (slopes NULL = no bias); key_mask[b, key] != 0 sets the score to
  *   "finfo.min" (a fully masked row attends uniformly); softmax and P.V in fp32, o stored as bf16.
  *   q: [batch, heads*head_dim] rows (q_bstride), k/v: [batch, nk, heads*head_dim] (shared kv_bstride and row stride
@@ -192,7 +193,8 @@ int ofk_attn_dense_bwd(const void* q, const void* k, const void* v, const void* 
  *   initialisation.  The workspace-size function returns OFK_ERR_ARG for arguments the kernel would reject.
  * The key split is a pure function of (batch, heads, head_dim, nk, SM count) and partials are merged in a fixed order
  * without atomics: the output is bitwise identical from launch to launch and does not depend on the cache's capacity.
- * Requirements: head_dim 64 or 128; batch, heads, nk >= 1 (OFK_ERR_ARG); q, k, v, o, key_mask and workspace 16-byte
+ * head_dim 80 (GPT-NeoX, RedPajama-INCITE-3B) runs on the same kernel with 16 lanes per key row, 10 of them loading.
+ * Requirements: head_dim 64, 80 or 128; batch, heads, nk >= 1 (OFK_ERR_ARG); q, k, v, o, key_mask and workspace 16-byte
  * aligned, every batch or row stride a multiple of 8 elements (OFK_ERR_ALIGN).  Every argument is checked before the
  * first CUDA call. */
 long long ofk_attn_decode_workspace_bytes(int batch, int heads, int head_dim, int nk);
@@ -228,6 +230,40 @@ int ofk_kv_append(const void* src, long long src_bstride, void* cache, long long
                   long long mask_bstride, const unsigned char* new_masked, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Rotary q/k packing of the GPT-NeoX decoder blocks (HF GPTNeoXAttention: apply_rotary_pos_emb on the rotate_half
+ * form), csrc/rope.cu.  The query_key_value Linear emits rows of `heads` heads, each (q | k | v) of head_dim columns.
+ *
+ * ofk_rope_pack: for each part p in (q, k, v) whose source is non-NULL, reads head h of row (b, t) at
+ *   src_p + b * src_bstride + t * ld_src + h * src_head_stride  (head_dim columns; the three parts share the strides)
+ * and writes it to  dst_p + b * p_bstride + t * ldp + h * p_width, columns [head_dim, p_width) zero.  For q and k the
+ * first `rot` columns are rotated:  y[j] = x[j] * cos[j] + rotate_half(x)[j] * sin[j]  with the product and the sum in
+ * fp32 (not fused) and one rounding to bf16, as autocast rounds HF's module; the other columns are bit copies.
+ *   cos, sin: f32 at  b * cs_bstride + t * ld_cs + j  (cs_bstride 0 = one table for every batch entry).  rot = 0 turns
+ *   the rotation off and cos/sin may be NULL: the kernel then only re-lays heads out (e.g. pads cached K/V rows, whose
+ *   K and V are two sources with head stride head_dim).
+ *   The interleaved QKV GEMM output is src_q = qkv, src_k = qkv + head_dim, src_v = qkv + 2 * head_dim with head
+ *   stride 3 * head_dim.
+ * ofk_rope_unpack_bwd: the adjoint.  From dq, dk, dv (heads of `width` columns, padding not read) writes the gradient
+ *   of the interleaved rows  dqkv[b, t, h * 3 * head_dim + p * head_dim + j],  with the transposed rotation
+ *   dx = dy * cos + rotate_half^T(dy * sin),  rotate_half^T(u) = (u[rot/2 .. rot), -u[0 .. rot/2)),  fp32, one rounding.
+ * Requirements: batch, rows, heads >= 1, head_dim a positive multiple of 8, rot even in [0, head_dim], cos and sin
+ *   non-NULL with cs_bstride >= 0 and ld_cs >= rot when rot > 0, every width >= head_dim and a multiple of 8, every
+ *   destination row stride >= heads * width (dqkv: >= 3 * heads * head_dim), src_head_stride >= head_dim, at least one
+ *   source and a destination for each (OFK_ERR_ARG); bf16 operands 16-byte aligned with every stride a multiple of 8
+ *   elements, cos and sin 4-byte aligned (OFK_ERR_ALIGN).  Every argument is checked before the first CUDA call.
+ */
+int ofk_rope_pack(const void* src_q, const void* src_k, const void* src_v, long long src_bstride, long long ld_src,
+                  int src_head_stride, int batch, int rows, int heads, int head_dim, int rot, const float* cos,
+                  const float* sin, long long cs_bstride, long long ld_cs, void* q, long long q_bstride, long long ldq,
+                  int q_width, void* k, long long k_bstride, long long ldk, int k_width, void* v, long long v_bstride,
+                  long long ldv, int v_width, void* stream);
+int ofk_rope_unpack_bwd(const void* dq, long long dq_bstride, long long lddq, const void* dk, long long dk_bstride,
+                        long long lddk, const void* dv, long long dv_bstride, long long lddv, int width, int batch,
+                        int rows, int heads, int head_dim, int rot, const float* cos, const float* sin,
+                        long long cs_bstride, long long ld_cs, void* dqkv, long long dqkv_bstride, long long lddqkv,
+                        void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Small fused elementwise / reduction kernels.
  */
 /* text_time[b, t] = inclusive cumsum over t of (ids[b,t] == media_id)   (helpers.py:208; flamingo.py:310)
@@ -259,6 +295,11 @@ long long ofk_reduce_workspace_bytes(void);
  * (OFK_ERR_ALIGN). */
 int ofk_gate_bwd(const float* dout, const void* branch, const float* gate, void* dbranch, float* dgate,
                  long long n, float* workspace, void* stream);
+
+/* h(bf16) = gelu_erf(z(bf16)), n elements, with the GELU of the BIAS_GELU_BF16 epilogue: a BIAS_BF16 GEMM followed by this
+ * gives the bits of a BIAS_GELU_BF16 GEMM and keeps z for the DGELU_BF16 backward (HF GPTNeoXMLP under autocast).
+ * n % 8 == 0 (OFK_ERR_ARG); z and h 16-byte aligned (OFK_ERR_ALIGN). */
+int ofk_gelu_bf16(const void* z, void* h, long long n, void* stream);
 
 /* dst(f32) += src(f32) */
 int ofk_add_f32(float* dst, const float* src, long long n, void* stream);

@@ -1,5 +1,5 @@
 // Decode attention of the frozen LM's decoder blocks with a KV cache: one query row per (batch, head) against the
-// first nk rows of a K/V cache, head_dim 64 or 128, bf16 in/out, fp32 softmax and P.V.  Semantics are those of
+// first nk rows of a K/V cache, head_dim 64, 80 or 128, bf16 in/out, fp32 softmax and P.V.  Semantics are those of
 // ofk_attn_dense_fwd at nq = 1:
 //
 //   S = scale * q K^T + slope[h] * key_index          (ALiBi; softmax is invariant to MPT's per-row constant)
@@ -7,8 +7,11 @@
 //   o = softmax(S) V
 //
 // At nq = 1 the products are matrix-vector, so tensor cores do not help (MPT is plain multi-head attention) and the
-// kernel is bound by reading K and V.  Each key row is read once, by C = head_dim / 8 threads with one 16-byte load
-// each; a CTA of 128 threads holds 128 / C key groups, and every group keeps UNROLL keys of K and V in flight.
+// kernel is bound by reading K and V.  Each key row is read once, by head_dim / 8 threads with one 16-byte load
+// each.  A key group is C lanes, head_dim / 8 rounded up to a power of two, so that a group is an aligned part of a
+// warp and its dot product sums in a shuffle tree; at head_dim 80 (GPT-NeoX, 10 loads per row) lanes 10..15 of each
+// 16-lane group load nothing and add zeros.  A CTA of 128 threads holds 128 / C key groups, and every group keeps
+// UNROLL keys of K and V in flight.
 // Split-KV ("flash-decoding"): the keys are cut into `nsplit` contiguous chunks, one CTA per (split, head, batch), so
 // that a small batch x heads still fills the GPU.  Each CTA merges its groups' (max, sum, acc) in shared memory in a
 // fixed order and writes one partial; a second kernel merges the partials in split order.  The split count is a pure
@@ -97,7 +100,9 @@ __device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
 
 template <int HD>
 __global__ void __launch_bounds__(THREADS) kv_decode_split_kernel(const Params p) {
-  constexpr int C = HD / 8;           // threads per key row
+  constexpr int CV = HD / 8;                      // threads that load a key row
+  constexpr int C = CV <= 8 ? 8 : 16;             // lanes per key group, a power of two
+  static_assert(HD % 8 == 0 && CV <= C, "head_dim must be a multiple of 8 and at most 128");
   constexpr int NG = THREADS / C;     // key groups per CTA
   constexpr int STEP = NG * UNROLL;   // keys per CTA iteration
   __shared__ float s_m[NG], s_l[NG];
@@ -105,13 +110,14 @@ __global__ void __launch_bounds__(THREADS) kv_decode_split_kernel(const Params p
 
   const int split = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int grp = threadIdx.x / C, c = threadIdx.x % C;
+  const bool active = c < CV;         // lanes past the row's last 16-byte piece hold zeros
   int nk, chunk, nsplit;
   plan(p, (long long)gridDim.z * p.heads, &nk, &chunk, &nsplit);
   if (split >= nsplit) return;   // uniform over the CTA, before any barrier
   const int k0 = split * chunk, k1 = min(nk, k0 + chunk);
 
   float qf[8];
-  unpack8(*reinterpret_cast<const uint4*>(p.q + b * p.q_bs + h * HD + c * 8), qf);
+  unpack8(active ? *reinterpret_cast<const uint4*>(p.q + b * p.q_bs + h * HD + c * 8) : make_uint4(0u, 0u, 0u, 0u), qf);
   const __nv_bfloat16* kp = p.k + b * p.kv_bs + h * HD + c * 8;
   const __nv_bfloat16* vp = p.v + b * p.kv_bs + h * HD + c * 8;
   const unsigned char* mp = p.mask != nullptr ? p.mask + b * p.mask_bs : nullptr;
@@ -131,8 +137,10 @@ __global__ void __launch_bounds__(THREADS) kv_decode_split_kernel(const Params p
       kr[u] = vr[u] = make_uint4(0u, 0u, 0u, 0u);
       msk[u] = false;
       if (key < k1) {
-        kr[u] = __ldg(reinterpret_cast<const uint4*>(kp + key * p.ldkv));
-        vr[u] = __ldg(reinterpret_cast<const uint4*>(vp + key * p.ldkv));
+        if (active) {
+          kr[u] = __ldg(reinterpret_cast<const uint4*>(kp + key * p.ldkv));
+          vr[u] = __ldg(reinterpret_cast<const uint4*>(vp + key * p.ldkv));
+        }
         if (mp != nullptr) msk[u] = mp[key] != 0;
       }
     }
@@ -171,8 +179,10 @@ __global__ void __launch_bounds__(THREADS) kv_decode_split_kernel(const Params p
 
   // merge the key groups in group order
   if (c == 0) { s_m[grp] = m; s_l[grp] = l; }
+  if (active) {
 #pragma unroll
-  for (int i = 0; i < 8; ++i) s_acc[grp][c * 8 + i] = acc[i];
+    for (int i = 0; i < 8; ++i) s_acc[grp][c * 8 + i] = acc[i];
+  }
   __syncthreads();
   if (threadIdx.x < HD) {
     const int d = threadIdx.x;
@@ -244,7 +254,8 @@ static int check_decode_args(const void* q, long long q_bstride, const void* k, 
                              long long ldkv, const void* o, long long o_bstride, int batch, int heads, int head_dim,
                              int nk, const unsigned char* key_mask, long long mask_bstride, const void* workspace) {
   if (!q || !k || !v || !o || !workspace) return ofk_set_error(OFK_ERR_ARG, "attention decode: null pointer");
-  if (head_dim != 64 && head_dim != 128) return ofk_set_error(OFK_ERR_ARG, "attention decode: head_dim must be 64 or 128");
+  if (head_dim != 64 && head_dim != 80 && head_dim != 128)
+    return ofk_set_error(OFK_ERR_ARG, "attention decode: head_dim must be 64, 80 or 128");
   if (batch < 1 || heads < 1 || nk < 1) return ofk_set_error(OFK_ERR_ARG, "attention decode: empty problem");
   if (batch > 65535 || heads > 65535) return ofk_set_error(OFK_ERR_ARG, "attention decode: batch/heads exceed grid limits");
   if (misaligned(q) || misaligned(k) || misaligned(v) || misaligned(o) || misaligned(workspace) ||
@@ -278,7 +289,7 @@ static Params make_params(const void* q, long long q_bstride, const void* k, con
 
 // grid_splits: the split kernel's grid width (the plan's split count, or its upper bound for a device key count).
 template <int HD>
-static int launch(const Params& p, int batch, int grid_splits, bool always_combine, cudaStream_t s) {
+static int launch_hd(const Params& p, int batch, int grid_splits, bool always_combine, cudaStream_t s) {
   kv_decode_split_kernel<HD><<<dim3(grid_splits, p.heads, batch), THREADS, 0, s>>>(p);
   OFK_CHECK_LAUNCH();
   if (always_combine || p.nsplit > 1) {
@@ -288,12 +299,18 @@ static int launch(const Params& p, int batch, int grid_splits, bool always_combi
   return 0;
 }
 
+static int launch(int head_dim, const Params& p, int batch, int grid_splits, bool always_combine, cudaStream_t s) {
+  if (head_dim == 64) return launch_hd<64>(p, batch, grid_splits, always_combine, s);
+  if (head_dim == 80) return launch_hd<80>(p, batch, grid_splits, always_combine, s);
+  return launch_hd<128>(p, batch, grid_splits, always_combine, s);
+}
+
 }  // namespace decode
 }  // namespace ofk
 
 extern "C" long long ofk_attn_decode_workspace_bytes(int batch, int heads, int head_dim, int nk) {
   using namespace ofk::decode;
-  if ((head_dim != 64 && head_dim != 128) || batch < 1 || heads < 1 || nk < 1) return OFK_ERR_ARG;
+  if ((head_dim != 64 && head_dim != 80 && head_dim != 128) || batch < 1 || heads < 1 || nk < 1) return OFK_ERR_ARG;
   const long long splits = std::min(MAX_SPLITS, (nk + MIN_CHUNK - 1) / MIN_CHUNK);
   return (long long)batch * heads * splits * (head_dim + 2) * (long long)sizeof(float);
 }
@@ -311,7 +328,7 @@ extern "C" int ofk_attn_decode(const void* q, long long q_bstride, const void* k
                          slopes, workspace);
   p.nsplit = split_count((long long)batch * heads, nk, sms, &p.chunk);
   cudaStream_t s = (cudaStream_t)stream;
-  return head_dim == 64 ? launch<64>(p, batch, p.nsplit, false, s) : launch<128>(p, batch, p.nsplit, false, s);
+  return launch(head_dim, p, batch, p.nsplit, false, s);
 }
 
 extern "C" int ofk_attn_decode_dev(const void* q, long long q_bstride, const void* k, const void* v,
@@ -334,7 +351,7 @@ extern "C" int ofk_attn_decode_dev(const void* q, long long q_bstride, const voi
   p.num_sms = sms;
   const int grid = max_split_count((long long)batch * heads, nk_max, sms);
   cudaStream_t s = (cudaStream_t)stream;
-  return head_dim == 64 ? launch<64>(p, batch, grid, true, s) : launch<128>(p, batch, grid, true, s);
+  return launch(head_dim, p, batch, grid, true, s);
 }
 
 extern "C" int ofk_kv_append(const void* src, long long src_bstride, void* cache, long long cache_bstride,

@@ -94,6 +94,20 @@ __global__ void cast_f32_bf16_kernel(const float* __restrict__ src, __nv_bfloat1
     dst[i] = __float2bfloat16_rn(src[i]);
 }
 
+// h = bf16(gelu_erf(z)) of a bf16 pre-activation, with the device function of the BIAS_GELU_BF16 GEMM epilogue: a
+// block that keeps z for the DGELU_BF16 backward takes z from a BIAS_BF16 GEMM and h from here, bit for bit what
+// BIAS_GELU_BF16 would have stored.
+__global__ void gelu_bf16_kernel(const uint4* __restrict__ z, uint4* __restrict__ h, long long n8) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += stride) {
+    const uint4 u = z[i];
+    h[i] = make_uint4(pack_bf16x2(gelu_exact(bf16_lo(u.x)), gelu_exact(bf16_hi(u.x))),
+                      pack_bf16x2(gelu_exact(bf16_lo(u.y)), gelu_exact(bf16_hi(u.y))),
+                      pack_bf16x2(gelu_exact(bf16_lo(u.z)), gelu_exact(bf16_hi(u.z))),
+                      pack_bf16x2(gelu_exact(bf16_lo(u.w)), gelu_exact(bf16_hi(u.w))));
+  }
+}
+
 // ---- gate backward: dbranch = dout * tanh(g) (bf16); dgate += (1 - tanh(g)^2) * <dout, branch>
 __global__ void __launch_bounds__(256) gate_bwd_kernel(const float* __restrict__ dout, const __nv_bfloat16* __restrict__ branch,
                                                        const float* __restrict__ gate, __nv_bfloat16* __restrict__ dbranch,
@@ -282,6 +296,16 @@ extern "C" int ofk_cast_f32_bf16(const float* src, void* dst, long long n, void*
   if ((reinterpret_cast<uintptr_t>(src) & 15) || (reinterpret_cast<uintptr_t>(dst) & 15))
     return ofk_set_error(OFK_ERR_ALIGN, "cast: pointers must be 16-byte aligned");
   cast_f32_bf16_kernel<<<grid_for(n / 8 + 1, 256), 256, 0, (cudaStream_t)stream>>>(src, (__nv_bfloat16*)dst, n);
+  OFK_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int ofk_gelu_bf16(const void* z, void* h, long long n, void* stream) {
+  if (!z || !h) return ofk_set_error(OFK_ERR_ARG, "gelu: null pointer");
+  if (n <= 0) return 0;
+  if (n % 8 != 0) return ofk_set_error(OFK_ERR_ARG, "gelu: n must be a multiple of 8");
+  if (misaligned(z, 16) || misaligned(h, 16)) return ofk_set_error(OFK_ERR_ALIGN, "gelu: pointers must be 16-byte aligned");
+  gelu_bf16_kernel<<<grid_for(n / 8, 256), 256, 0, (cudaStream_t)stream>>>((const uint4*)z, (uint4*)h, n / 8);
   OFK_CHECK_LAUNCH();
   return 0;
 }

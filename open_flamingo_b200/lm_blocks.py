@@ -1,4 +1,5 @@
-"""Frozen-LM decoder blocks on the sm_90a kernels (SURVEY.md section 8f, rank 1).
+"""Frozen-LM decoder blocks on the sm_90a kernels (SURVEY.md section 8f, rank 1): HF `MptBlock` (OF-3B, OF-9B) and
+HF `GPTNeoXLayer` (OF-4B; see the GPT-NeoX section below).
 
 The reference runs the frozen LM's decoder block as ordinary PyTorch (`self.decoder_layer(lang_x, ...)`,
 flamingo_lm.py:63-65).  For the LM family named by BASELINE.json (MPT: HF `MptBlock` = LN -> Wqkv -> causal
@@ -8,11 +9,12 @@ GELU / residual epilogues, LayerNorm, dense attention), forward plus the dgrad-o
 needs.
 
 Decoding with a KV cache runs on the kernels too when the cache is a kv_cache.KVCache and no gradient is recorded
-(`no_grad` / `inference_mode`): the K/V projection GEMM writes the new rows straight into the cache buffer, one new
-token attends through the split-KV decode kernel (ops.attn_decode) and a multi-token chunk (prefill, or a chunk after a
-prefix) through the dense kernel over the cached keys.  Anything else -- other LM families, HF's DynamicCache, dropout,
-clip_qkv, output_attentions -- takes the block's own PyTorch forward, exactly as in the reference (a block that declines
-still reads and extends a KVCache through HF's `MptAttention` and `KVCache.update`).
+(`no_grad` / `inference_mode`): the K/V projection GEMM (GPT-NeoX: the rotary packing) writes the new rows straight
+into the cache buffer, one new token attends through the split-KV decode kernel (ops.attn_decode) and a multi-token
+chunk (prefill, or a chunk after a prefix) through the dense kernel over the cached keys.  Anything else -- other LM
+families, HF's DynamicCache, dropout, clip_qkv, output_attentions (GPT-NeoX: also output_hidden_states, which HF
+records with hooks on the layer modules) -- takes the block's own PyTorch forward, exactly as in the reference (a
+block that declines still reads and extends a KVCache through HF's attention module and `KVCache.update`).
 
 Numerics are those of the block under `torch.autocast(bfloat16)`: fp32 residual stream, fp32 LayerNorm/softmax,
 bf16 GEMM operands, bf16 K/V cache.
@@ -32,8 +34,8 @@ f32 = torch.float32
 ENABLED = True  # module-level switch (bench.py --lm eager turns it off to time the reference's PyTorch LM path)
 
 _zero_bias = {}
-# (weakref to HF's [B,1,T,nk] bool mask, its byte form for the kernels, whether that is the decode form) -- converted
-# once per forward and shared by every block
+# (weakref to HF's [B,1,T,nk] bool mask, its byte form for the kernels, (whether that is the decode form, whether True
+# meant "attend")) -- converted once per forward and shared by every block
 _mask_cache = [None, None, None]
 
 
@@ -44,6 +46,26 @@ def _zeros(n, device):
         t = torch.zeros(n, device=device, dtype=f32)
         _zero_bias[key] = t
     return t
+
+
+def _kernel_mask(m, B, T, nk, decode, true_attends=False):
+    """HF's 4-D bool mask `m` [1 or B, 1, T, nk] as the kernels' bytes (nonzero = masked), or None if `m` is not such a
+    mask.  decode: key padding only, [B, nk rounded up to 8] for the decode kernel; else [B, T, nk].  true_attends: True
+    in `m` means "attend" (HF's sdpa mask for GPT-NeoX) rather than "masked" (MPT)."""
+    if m.dtype != torch.bool or m.dim() != 4 or m.shape[0] not in (1, B) or m.shape[1] != 1 or m.shape[2] != T or \
+            m.shape[3] != nk:
+        return None
+    ref = _mask_cache[0]
+    if ref is not None and ref() is m and _mask_cache[1].shape[0] == B and _mask_cache[2] == (decode, true_attends):
+        return _mask_cache[1]
+    m_masked = ~m if true_attends else m
+    if decode:   # key padding only, rows padded to a multiple of 8 bytes for the decode kernel
+        mask = torch.zeros((B, -(-nk // 8) * 8), dtype=torch.uint8, device=m.device)
+        mask[:, :nk].copy_(m_masked.expand(B, 1, 1, nk).reshape(B, nk))
+    else:
+        mask = m_masked.expand(B, 1, T, nk).reshape(B, T, nk).contiguous()
+    _mask_cache[0], _mask_cache[1], _mask_cache[2] = weakref.ref(m), mask, (decode, true_attends)
+    return mask
 
 
 def _block_tail(x2d, o, eps, wout, n2_w, wup, wdown):
@@ -276,20 +298,9 @@ class FastMptBlock:
         decode = layer is not None and T == 1
         mask = None
         if attention_mask is not None:
-            m = attention_mask
-            if m.dtype != torch.bool or m.dim() != 4 or m.shape[0] not in (1, B) or m.shape[1] != 1 or \
-                    m.shape[2] != T or m.shape[3] != nk:
+            mask = _kernel_mask(attention_mask, B, T, nk, decode)
+            if mask is None:
                 return None
-            ref = _mask_cache[0]
-            if ref is not None and ref() is m and _mask_cache[1].shape[0] == B and _mask_cache[2] == decode:
-                mask = _mask_cache[1]
-            else:
-                if decode:   # key padding only, rows padded to a multiple of 8 bytes for the decode kernel
-                    mask = torch.zeros((B, -(-nk // 8) * 8), dtype=torch.uint8, device=m.device)
-                    mask[:, :nk].copy_(m.expand(B, 1, 1, nk).reshape(B, nk))
-                else:
-                    mask = m.expand(B, 1, T, nk).reshape(B, T, nk).contiguous()
-                _mask_cache[0], _mask_cache[1], _mask_cache[2] = weakref.ref(m), mask, decode
         x = hidden_states if hidden_states.dtype == f32 else hidden_states.float()
         weights = self.weights()
         flag = pure_causal_flag if mask is not None else None
@@ -302,8 +313,281 @@ class FastMptBlock:
         return out, None
 
 
+# ---- GPT-NeoX (HF GPTNeoXLayer: OpenFlamingo-4B's RedPajama-INCITE-3B) ------------------------------------------------
+#
+#   a = LN1(x);  qkv = a Wqkv^T + bqkv  (heads interleaved as (q | k | v));  q, k = rotary(q, k; cos, sin)
+#   y = softmax(q k^T / sqrt(hd) + mask) v Wd^T + bd
+#   sequential: x1 = y + x,  out = MLP(LN2(x1)) + x1;   parallel: out = MLP(LN2(x)) + y + x
+#   MLP(u) = gelu_erf(u W1^T + b1) W2^T + b2
+#
+# The attention cores exist for head_dim 64 and 128.  Other head_dims (80 for RedPajama-INCITE-3B: D 2560, 32 heads) run
+# on the 128 cores with every head zero-padded to 128 columns: ops.rope_pack writes the rotated q, k and v in that
+# layout, zero columns add exact zeros to q k^T, to P v and to every backward product, so the result is the head_dim-80
+# attention.  The attention output then has H * 128 columns; the out-projection reads it through a copy of Wd with the
+# same zero columns (_padded_w16), and in the backward the dgrad GEMM with that copy yields the padded d_o directly.
+# Decoding one token runs the decode kernel at head_dim 80 directly, on an unpadded KV cache.
+
+
+def _neox_width(hd):
+    """Head width the attention cores run a head_dim-hd head at."""
+    return hd if hd in (64, 128) else 128
+
+
+_wpad_cache = {}
+
+
+def _padded_w16(param, heads, hd, width):
+    """bf16 copy of an out-projection weight [D, heads * hd] with each head's columns zero-padded to `width`:
+    [D, heads * width].  Refreshed by w16's rule -- a weakly referenced parameter at the same version counter and
+    address -- so `load_state_dict` or an in-place edit is seen."""
+    if width == hd:
+        return w16(param)
+    key = id(param)
+    ent = _wpad_cache.get(key)
+    if ent is not None and ent[0]() is param and ent[1] == param._version and ent[2] == param.data_ptr():
+        return ent[3]
+    D = param.shape[0]
+    t = torch.zeros((D, heads, width), device=param.device, dtype=bf16)
+    t[..., :hd].copy_(w16(param).view(D, heads, hd))   # a layout change of the bf16 copy, made once per weight version
+    t = t.view(D, heads * width)
+    _wpad_cache[key] = (weakref.ref(param, lambda _r, k=key: _wpad_cache.pop(k, None)), param._version,
+                        param.data_ptr(), t)
+    return t
+
+
+def _neox_tail(x2d, o, parallel, eps2, wout16, bd, n2_w, n2_b, w1, b1, w2, b2, keep_z):
+    """The block after its attention core.  x2d: [R, D] f32 block input; o: [R, heads * width] bf16 attention output;
+    wout16: the bf16 out-projection weight for that width.  Returns (out, x1, mean2, rstd2, z): x1 = bf16(y) + x, the
+    LayerNorm-2 statistics (of x1, or of x in the parallel form) and the bf16 pre-activation z (None unless keep_z).
+
+    The parallel form adds bf16(y) and bf16(mlp) to the fp32 stream one after the other; autocast adds them in bf16
+    first, so this is the more precise of the two (by at most one bf16 rounding of y + mlp)."""
+    x1 = ops.gemm(o, wout16, epi=L.EPI_BIAS_RESID_F32, bias=bd, aux=x2d)
+    un, mean2, rstd2 = ops.layernorm_fwd(x2d if parallel else x1, n2_w, n2_b, eps2, want_stats=keep_z)
+    if keep_z:   # z for the DGELU_BF16 backward; gelu_bf16 gives the bits BIAS_GELU_BF16 would
+        z = ops.gemm(un, w16(w1), epi=L.EPI_BIAS_BF16, bias=b1)
+        h = ops.gelu_bf16(z)
+    else:
+        z = None
+        h = ops.gemm(un, w16(w1), epi=L.EPI_BIAS_GELU_BF16, bias=b1)
+    del un
+    out = ops.gemm(h, w16(w2), epi=L.EPI_BIAS_RESID_F32, bias=b2, aux=x1)
+    return out, x1, mean2, rstd2, z
+
+
+def _rows(x):
+    B, T, D = x.shape
+    x2d = x.reshape(B * T, D)
+    return x2d if x2d.is_contiguous() else x2d.contiguous()
+
+
+class FrozenNeoXBlockFn(torch.autograd.Function):
+    """A frozen GPTNeoXLayer: forward, and the backward to its input only (the parameters take no gradient).
+    x: [B, T, D] f32; mask: [B, T, T] bytes (nonzero = masked) or None for causal only; cos, sin: f32 [1 or B, T, rot]."""
+
+    @staticmethod
+    def forward(ctx, x, mask, pure_flag, cos, sin, heads, parallel, eps1, eps2, n1_w, n1_b, wqkv, bqkv, wd, bd, n2_w,
+                n2_b, w1, b1, w2, b2):
+        B, T, D = x.shape
+        R = B * T
+        hd = D // heads
+        W = _neox_width(hd)
+        x2d = _rows(x)
+        xn, mean1, rstd1 = ops.layernorm_fwd(x2d, n1_w, n1_b, eps1)
+        qkv = ops.gemm(xn, w16(wqkv), epi=L.EPI_BIAS_BF16, bias=bqkv)                # [R, 3D]
+        del xn
+        q, k, v = ops.rope_pack(qkv.view(B, T, 3 * D), heads, hd, cos, sin, q_width=W, kv_width=W)
+        del qkv
+        scale = float(hd ** -0.5)
+        o, lse = ops.attn_dense_fwd(q, k, v, heads, W, scale, causal=mask is None, mask=mask,
+                                    pure_causal_flag=pure_flag)
+        out, x1, mean2, rstd2, z = _neox_tail(x2d, o.view(R, heads * W), parallel, eps2, _padded_w16(wd, heads, hd, W),
+                                              bd, n2_w, n2_b, w1, b1, w2, b2, keep_z=True)
+        ctx.save_for_backward(x2d, mean1, rstd1, q, k, v, o, lse, x1, mean2, rstd2, z, cos, sin, n1_w, wqkv, wd, n2_w,
+                              w1, w2, mask if mask is not None else x2d.new_empty(0),
+                              pure_flag if pure_flag is not None else x2d.new_empty(0))
+        ctx.meta = (B, T, D, heads, hd, W, scale, parallel, mask is not None, pure_flag is not None)
+        return out.view(B, T, D)
+
+    @staticmethod
+    def backward(ctx, dout):
+        (x2d, mean1, rstd1, q, k, v, o, lse, x1, mean2, rstd2, z, cos, sin, n1_w, wqkv, wd, n2_w, w1, w2, mask,
+         pure_flag) = ctx.saved_tensors
+        B, T, D, heads, hd, W, scale, parallel, has_mask, has_flag = ctx.meta
+        mask = mask if has_mask else None
+        pure_flag = pure_flag if has_flag else None
+        R = B * T
+        d2 = _rows(dout)
+        if d2.dtype != f32:
+            d2 = d2.float()
+        dbr = ops.gate_bwd(d2, None, None, None)                                     # bf16 cast
+        dz = ops.gemm(dbr, w16(w2), b_mn=True, epi=L.EPI_DGELU_BF16, aux=z)          # (d W2) * gelu'(z)
+        du = ops.gemm(dz, w16(w1), b_mn=True)
+        del dz
+        # d/dx1 (sequential) or the MLP branch's share of d/dx (parallel), plus the straight-through d2
+        dx1 = ops.layernorm_bwd(du, x2d if parallel else x1, n2_w, mean2, rstd2, dx_add=d2)
+        del du
+        dy = dbr if parallel else ops.gate_bwd(dx1, None, None, None)
+        d_o = ops.gemm(dy, _padded_w16(wd, heads, hd, W), b_mn=True)                # [R, heads * W], padding zero
+        del dy, dbr
+        dq, dk, dv = ops.attn_dense_bwd(q, k, v, o, d_o.view(B, T, heads * W), lse, heads, W, scale,
+                                        causal=mask is None, mask=mask, pure_causal_flag=pure_flag)
+        del d_o
+        dqkv = ops.rope_unpack_bwd(dq, dk, dv, heads, hd, cos, sin)                  # [B, T, 3D]
+        del dq, dk, dv
+        dxn = ops.gemm(dqkv.view(R, 3 * D), w16(wqkv), b_mn=True)
+        dx = ops.layernorm_bwd(dxn, x2d, n1_w, mean1, rstd1, dx_add=dx1)
+        return (dx.view(B, T, D),) + (None,) * 20
+
+
+def cached_neox_block_forward(x, layer, mask, pure_flag, cos, sin, heads, parallel, eps1, eps2, n1_w, n1_b, wqkv, bqkv,
+                              wd, bd, n2_w, n2_b, w1, b1, w2, b2):
+    """Inference forward of one GPT-NeoX block that appends its nq new tokens to `layer` (a kv_cache.KVCacheLayer,
+    unpadded head_dim rows, so HF's attention can extend it through KVCacheLayer.update) and attends over everything
+    cached.  ops.rope_pack writes the rotated K and the V straight into cache rows [past, past + nq).
+      nq == 1: q unpadded, the decode kernel at head_dim hd, the out-projection with Wd itself;
+      nq > 1 : q and the cached K/V rows [0, nk) padded to the core's width, the dense kernel, the padded Wd.
+    mask: as for cached_block_forward.  x: [B, nq, D] f32; returns the same."""
+    B, nq, D = x.shape
+    hd = D // heads
+    x2d = _rows(x)
+    xn, _, _ = ops.layernorm_fwd(x2d, n1_w, n1_b, eps1, want_stats=False)
+    qkv = ops.gemm(xn, w16(wqkv), epi=L.EPI_BIAS_BF16, bias=bqkv).view(B, nq, 3 * D)
+    del xn
+    if not layer.is_initialized:
+        layer.init_storage(B, heads, hd, bf16, x.device)
+    past = layer.length
+    rows = layer.reserve(nq)[:, past:past + nq]
+    scale = float(hd ** -0.5)
+    W = hd if nq == 1 else _neox_width(hd)
+    q, _, _ = ops.rope_pack(qkv, heads, hd, cos, sin, q_width=W, k=rows[..., :D], v=rows[..., D:])
+    del qkv
+    layer.length = past + nq
+    k, v = layer.kv_views()
+    if nq == 1:
+        o = ops.attn_decode(q.view(B, D), k, v, heads, hd, scale, key_mask=mask)
+    else:
+        if W != hd:
+            _, k, v = ops.rope_pack(None, heads, hd, kv_src=(k, v), kv_width=W)
+        o, _ = ops.attn_dense_fwd(q, k, v, heads, W, scale, causal=mask is None, mask=mask, pure_causal_flag=pure_flag,
+                                  want_lse=False)
+    return _neox_tail(x2d, o.view(B * nq, heads * W), parallel, eps2, _padded_w16(wd, heads, hd, W), bd, n2_w, n2_b,
+                      w1, b1, w2, b2, keep_z=False)[0].view(B, nq, D)
+
+
+class FastNeoXBlock:
+    """Callable with HF GPTNeoXLayer.forward's signature; returns None when the fast path does not apply, and the
+    block's output tensor otherwise."""
+
+    def __init__(self, block):
+        self.block = block
+
+    def records_outputs(self, output_attentions=None, output_hidden_states=None):
+        """Whether the caller asked HF to record this layer's hidden states or attention weights.  GPTNeoXModel
+        records both with hooks on the GPTNeoXLayer and GPTNeoXAttention modules, which the fast path does not call,
+        so such a call must run HF's layer.  An explicit keyword wins; without one the model config's default holds,
+        as in HF's capture_outputs."""
+        cfg = self.block.attention.config
+        if output_attentions is None:
+            output_attentions = getattr(cfg, "output_attentions", False)
+        if output_hidden_states is None:
+            output_hidden_states = getattr(cfg, "output_hidden_states", False)
+        return bool(output_attentions or output_hidden_states)
+
+    def supported(self, hidden_states, position_embeddings, record_outputs):
+        """The block and call are ones the kernels evaluate, whatever the cache.  record_outputs: see
+        records_outputs."""
+        b = self.block
+        a = b.attention
+        if not ENABLED or not hidden_states.is_cuda or record_outputs or position_embeddings is None:
+            return False
+        cos, sin = position_embeddings
+        hd = a.head_size
+        if hd not in (64, 80, 128) or abs(a.scaling - hd ** -0.5) > 1e-9:
+            return False
+        if cos.dtype != f32 or sin.dtype != f32 or cos.dim() != 3 or cos.shape != sin.shape or \
+                cos.stride() != sin.stride() or cos.stride(2) != 1 or cos.shape[2] % 2 or not 0 < cos.shape[2] <= hd:
+            return False
+        if b.training and (a.attention_dropout > 0 or b.post_attention_dropout.p > 0 or b.post_mlp_dropout.p > 0):
+            return False
+        if getattr(a.config, "hidden_act", None) != "gelu":
+            return False
+        lins = (a.query_key_value, a.dense, b.mlp.dense_h_to_4h, b.mlp.dense_4h_to_h, b.input_layernorm,
+                b.post_attention_layernorm)
+        if any(m.bias is None for m in lins) or any(p.dtype != f32 for p in b.parameters()):
+            return False
+        if any(p.requires_grad for p in b.parameters()):
+            return False   # this path has no wgrad: frozen blocks only
+        return True
+
+    def weights(self):
+        b = self.block
+        a = b.attention
+        return (b.input_layernorm.weight, b.input_layernorm.bias, a.query_key_value.weight, a.query_key_value.bias,
+                a.dense.weight, a.dense.bias, b.post_attention_layernorm.weight, b.post_attention_layernorm.bias,
+                b.mlp.dense_h_to_4h.weight, b.mlp.dense_h_to_4h.bias, b.mlp.dense_4h_to_h.weight,
+                b.mlp.dense_4h_to_h.bias)
+
+    def applicable(self, hidden_states, position_embeddings, layer_past, use_cache, record_outputs):
+        """The uncached path (FrozenNeoXBlockFn, forward and backward)."""
+        if layer_past is not None or use_cache:
+            return False
+        return self.supported(hidden_states, position_embeddings, record_outputs)
+
+    def cache_layer(self, hidden_states, position_embeddings, layer_past, record_outputs):
+        """The KVCacheLayer the cached path appends to, or None (see FastMptBlock.cache_layer)."""
+        if not isinstance(layer_past, KVCache) or torch.is_grad_enabled():
+            return None
+        if not self.supported(hidden_states, position_embeddings, record_outputs):
+            return None
+        a = self.block.attention
+        if a.layer_idx is None or not 0 <= a.layer_idx < len(layer_past.layers):
+            return None
+        layer = layer_past.layers[a.layer_idx]
+        if layer.is_initialized and (layer.buf.dtype != bf16 or layer.buf.device != hidden_states.device or
+                                     layer.buf.shape[0] != hidden_states.shape[0] or
+                                     layer.heads != a.config.num_attention_heads or layer.head_dim != a.head_size):
+            return None
+        return layer
+
+    def __call__(self, hidden_states, attention_mask=None, position_ids=None, use_cache=False, layer_past=None,
+                 position_embeddings=None, output_attentions=None, output_hidden_states=None, pure_causal_flag=None,
+                 **kwargs):
+        record = self.records_outputs(output_attentions, output_hidden_states)
+        layer = None
+        if layer_past is not None or use_cache:
+            layer = self.cache_layer(hidden_states, position_embeddings, layer_past, record)
+            if layer is None:
+                return None
+        elif not self.applicable(hidden_states, position_embeddings, layer_past, use_cache, record):
+            return None
+        b = self.block
+        B, T, _ = hidden_states.shape
+        cos, sin = position_embeddings
+        if cos.shape[0] not in (1, B) or cos.shape[1] != T:
+            return None
+        nk = T if layer is None else layer.length + T
+        mask = None
+        if attention_mask is not None:   # HF's sdpa mask, True = attend; a float (eager) mask is declined here
+            mask = _kernel_mask(attention_mask, B, T, nk, layer is not None and T == 1, true_attends=True)
+            if mask is None:
+                return None
+        x = hidden_states if hidden_states.dtype == f32 else hidden_states.float()
+        flag = pure_causal_flag if mask is not None else None
+        rest = (cos, sin, b.attention.config.num_attention_heads, bool(b.use_parallel_residual), b.input_layernorm.eps,
+                b.post_attention_layernorm.eps) + self.weights()
+        if layer is not None:
+            out = cached_neox_block_forward(x, layer, mask, flag, *rest)
+        else:
+            out = FrozenNeoXBlockFn.apply(x, mask, flag, *rest)
+        return out if out.dtype == hidden_states.dtype else out.to(hidden_states.dtype)
+
+
 def accelerate(decoder_layer):
-    """Return a fast evaluator for a recognised frozen decoder block, else None."""
-    if type(decoder_layer).__name__ == "MptBlock" and hasattr(decoder_layer, "attn") and hasattr(decoder_layer, "ffn"):
+    """Return a fast evaluator for a recognised frozen decoder block (HF MptBlock or GPTNeoXLayer), else None."""
+    name = type(decoder_layer).__name__
+    if name == "MptBlock" and hasattr(decoder_layer, "attn") and hasattr(decoder_layer, "ffn"):
         return FastMptBlock(decoder_layer)
+    if name == "GPTNeoXLayer" and hasattr(decoder_layer, "attention") and hasattr(decoder_layer, "mlp"):
+        return FastNeoXBlock(decoder_layer)
     return None

@@ -608,3 +608,107 @@ def gemm_grouped(a, b, *, a_mn=False, b_mn=False, epi=L.EPI_STORE_BF16, out, M, 
         out.data_ptr(), out.stride(0), L.ptr(bias), out_map[0], out_map[1], out_map[2], ak_map[0], ak_map[1], ak_map[2],
         L.stream_ptr()))
     return out
+
+
+def _rope_tables(cos, sin, B, rows, rot):
+    """(cs_bstride, ld_cs) of fp32 cos/sin tables [1 or B, rows, rot] with unit inner stride and equal strides."""
+    for t, name in ((cos, "cos"), (sin, "sin")):
+        if t.dtype != f32 or t.dim() != 3 or t.shape[0] not in (1, B) or t.shape[1] != rows or t.shape[2] != rot or \
+                t.stride(2) != 1:
+            raise ValueError(f"{name} must be float32 [1 or {B}, {rows}, {rot}] with unit inner stride, got "
+                             f"{tuple(t.shape)} {t.dtype} stride {t.stride()}")
+    if cos.shape != sin.shape or cos.stride() != sin.stride():
+        raise ValueError("cos and sin must have the same shape and strides")
+    return (cos.stride(0) if cos.shape[0] == B and B > 1 else 0), cos.stride(1)
+
+
+def _rope_dest(t, name, B, rows, inner):
+    if t.dtype != bf16 or t.dim() != 3 or tuple(t.shape) != (B, rows, inner) or t.stride(2) != 1:
+        raise ValueError(f"{name} must be a bf16 [{B}, {rows}, {inner}] view with unit inner stride, got "
+                         f"{tuple(t.shape)} {t.dtype} stride {t.stride()}")
+    return t.stride(0), t.stride(1)
+
+
+def rope_pack(src, heads, head_dim, cos=None, sin=None, *, q=None, k=None, v=None, q_width=None, kv_width=None,
+              kv_src=None):
+    """Rotary q/k packing of GPT-NeoX rows (ofk_rope_pack).
+
+    src: [B, T, heads * 3 * head_dim] bf16 view of the query_key_value output (heads interleaved as (q | k | v)), or
+    None with kv_src = (k_rows, v_rows): two [B, T, heads * head_dim] views (the K and V columns of a KV cache) whose
+    heads are only re-laid out.  cos/sin: fp32 [1 or B, T, rot] (None: no rotation).  q / k / v: destinations
+    [B, T, heads * width] (allocated when None and wanted); q_width, kv_width: head widths (default head_dim), columns
+    past head_dim are zero.  Returns (q, k, v); q is None with kv_src."""
+    L.require_cuda(src, cos, sin, q, k, v, *(kv_src or ()))
+    q_width = head_dim if q_width is None else q_width
+    kv_width = head_dim if kv_width is None else kv_width
+    if src is not None:
+        if src.dtype != bf16 or src.dim() != 3 or src.shape[2] != heads * 3 * head_dim or src.stride(2) != 1:
+            raise ValueError(f"src must be a bf16 [B, T, {heads * 3 * head_dim}] view with unit inner stride, got "
+                             f"{tuple(src.shape)} {src.dtype}")
+        B, T = src.shape[:2]
+        srcs = (src, src[..., head_dim:], src[..., 2 * head_dim:])
+        sbs, sld, shs = src.stride(0), src.stride(1), 3 * head_dim
+    else:
+        ks, vs = kv_src
+        if ks.dtype != bf16 or ks.dim() != 3 or ks.shape != vs.shape or ks.stride() != vs.stride() or \
+                ks.shape[2] != heads * head_dim or ks.stride(2) != 1:
+            raise ValueError(f"kv_src must be two bf16 [B, T, {heads * head_dim}] views with equal strides")
+        B, T = ks.shape[:2]
+        srcs = (None, ks, vs)
+        sbs, sld, shs = ks.stride(0), ks.stride(1), head_dim
+    rot = 0
+    cs_bs = ld_cs = 0
+    if cos is not None:
+        rot = cos.shape[-1]
+        cs_bs, ld_cs = _rope_tables(cos, sin, B, T, rot)
+    outs = []
+    for t, name, w, s in ((q, "q", q_width, srcs[0]), (k, "k", kv_width, srcs[1]), (v, "v", kv_width, srcs[2])):
+        if s is None:
+            outs.append((None, 0, 0, 0))
+            continue
+        if t is None:
+            t = torch.empty((B, T, heads * w), device=s.device, dtype=bf16)
+        outs.append((t,) + _rope_dest(t, name, B, T, heads * w) + (w,))
+    args = []
+    for t, bs, ld, w in outs:
+        args += [L.ptr(t), bs, ld, w]
+    L.check(L.lib().ofk_rope_pack(L.ptr(srcs[0]), L.ptr(srcs[1]), L.ptr(srcs[2]), sbs, sld, shs, B, T, heads, head_dim,
+                                  rot, L.ptr(cos), L.ptr(sin), cs_bs, ld_cs, *args, L.stream_ptr()))
+    return outs[0][0], outs[1][0], outs[2][0]
+
+
+def rope_unpack_bwd(dq, dk, dv, heads, head_dim, cos=None, sin=None, *, out=None):
+    """Adjoint of rope_pack (ofk_rope_unpack_bwd): dq/dk/dv [B, T, heads * W] bf16 views -> the gradient of the
+    interleaved rows, [B, T, heads * 3 * head_dim] bf16 (`out`, allocated when None)."""
+    L.require_cuda(dq, dk, dv, cos, sin, out)
+    if dq.dim() != 3 or dq.shape[2] % heads != 0:
+        raise ValueError(f"dq must be [B, T, heads * width], got {tuple(dq.shape)}")
+    B, T, inner = dq.shape
+    W = inner // heads
+    strides = []
+    for t, name in ((dq, "dq"), (dk, "dk"), (dv, "dv")):
+        strides += list(_rope_dest(t, name, B, T, inner))
+    rot = 0
+    cs_bs = ld_cs = 0
+    if cos is not None:
+        rot = cos.shape[-1]
+        cs_bs, ld_cs = _rope_tables(cos, sin, B, T, rot)
+    if out is None:
+        out = torch.empty((B, T, heads * 3 * head_dim), device=dq.device, dtype=bf16)
+    obs, old = _rope_dest(out, "out", B, T, heads * 3 * head_dim)
+    L.check(L.lib().ofk_rope_unpack_bwd(dq.data_ptr(), strides[0], strides[1], dk.data_ptr(), strides[2], strides[3],
+                                        dv.data_ptr(), strides[4], strides[5], W, B, T, heads, head_dim, rot,
+                                        L.ptr(cos), L.ptr(sin), cs_bs, ld_cs, out.data_ptr(), obs, old,
+                                        L.stream_ptr()))
+    return out
+
+
+def gelu_bf16(z, out=None):
+    """h = bf16(gelu_erf(z)) for a contiguous bf16 z, bit for bit the BIAS_GELU_BF16 epilogue's GELU."""
+    L.require_cuda(z, out)
+    _vector(z, "z", bf16, z.numel())
+    if out is None:
+        out = torch.empty(z.shape, device=z.device, dtype=bf16)
+    _vector(out, "out", bf16, z.numel())
+    L.check(L.lib().ofk_gelu_bf16(z.data_ptr(), out.data_ptr(), z.numel(), L.stream_ptr()))
+    return out

@@ -32,8 +32,8 @@ class FlamingoLayer(nn.Module):
         self.vis_x = None
         self.media_locations = None
         self.use_cached_media = None
-        # recognised frozen decoder blocks (HF MptBlock) are evaluated on the sm_90a kernels; everything else --
-        # and every case the fast path declines -- runs the block's own PyTorch forward as in the reference
+        # recognised frozen decoder blocks (HF MptBlock, GPTNeoXLayer) are evaluated on the sm_90a kernels; everything
+        # else -- and every case the fast path declines -- runs the block's own PyTorch forward as in the reference
         self._fast_block = lm_blocks.accelerate(decoder_layer)
         self._pure_causal_flag = None
         # kept for API compatibility (train.py:368-381); the fused blocks already store only what backward needs
@@ -57,8 +57,9 @@ class FlamingoLayer(nn.Module):
 
     def forward(self, lang_x, attention_mask=None, **decoder_layer_kwargs):
         """lang_x (B, T_txt, D) -> whatever the wrapped decoder block returns (flamingo_lm.py:43-66).  The gated
-        block runs on libofk (fused.GatedXattnBlockFn); a recognised frozen block too (lm_blocks.FrozenMptBlockFn),
-        falling back to the block's own PyTorch forward whenever the fast path declines (KV cache, dropout, ...)."""
+        block runs on libofk (fused.GatedXattnBlockFn); a recognised frozen block too (lm_blocks.FrozenMptBlockFn,
+        FrozenNeoXBlockFn), falling back to the block's own PyTorch forward whenever the fast path declines (KV cache,
+        dropout, ...)."""
         xattn = self.gated_cross_attn_layer
         if xattn is not None:
             # same failure modes as the reference (flamingo_lm.py:47-53)
@@ -166,8 +167,8 @@ class FlamingoLMMixin(nn.Module):
     def make_kv_cache(self, capacity=None):
         """A kv_cache.KVCache for decoding this LM on the kernels, or None where HF's own cache is kept: it is made only
         on CUDA, under `torch.autocast("cuda", dtype=torch.bfloat16)` (the caller asked for bf16 numerics; the cache
-        stores bf16), with lm_blocks.ENABLED, and when every decoder block is a recognised MPT block.  In fp32 every
-        path stays HF's.
+        stores bf16), with lm_blocks.ENABLED, and when every decoder block is a recognised MPT or GPT-NeoX block.  In
+        fp32 every path stays HF's.
 
         capacity: None for a cache that grows; an int for a fixed-capacity cache of at least that many rows, with which
         `forward(..., past_key_values=cache)` replays one captured CUDA graph per one-token step (decode_graph).  Its

@@ -56,15 +56,43 @@ def build_mpt(mpt_kw, dtype=torch.float32, device="cpu", seed=0):
     return lm.to(dtype).eval()
 
 
+# RedPajama-INCITE-3B (togethercomputer/RedPajama-INCITE-Base-3B-v1), the LM of OpenFlamingo-4B: D 2560, 32 heads of 80,
+# 32 layers, FFN 10240.  Full rotary and sequential residual are what we understand the release to use (not checked
+# against the hub config here).
+NEOX_3B = dict(hidden_size=2560, num_attention_heads=32, num_hidden_layers=32, intermediate_size=10240,
+               vocab_size=50432, max_position_embeddings=2048, rotary_pct=1.0, use_parallel_residual=False,
+               layer_norm_eps=1e-5)
+
+
+def build_neox(neox_kw, dtype=torch.float32, device="cpu", seed=0):
+    """Random-init HF GPTNeoXForCausalLM from a GPTNeoXConfig (offline).  `rotary_pct` sets the config's
+    partial_rotary_factor; the attention runs through sdpa (HF's default), whose boolean mask is what the kernels
+    take."""
+    from transformers import GPTNeoXConfig, GPTNeoXForCausalLM
+    torch.manual_seed(seed)
+    kw = dict(neox_kw)
+    rot = kw.pop("rotary_pct", 1.0)
+    cfg = GPTNeoXConfig(**kw, attn_implementation="sdpa")
+    cfg.rope_parameters["partial_rotary_factor"] = rot
+    with torch.device(device):
+        lm = GPTNeoXForCausalLM(cfg)
+    return lm.to(dtype).eval()
+
+
 def build_flamingo(vit_cfg, mpt_kw, cross_attn_every_n_layers=1, device="cuda", freeze_lm_embeddings=True, seed=0,
-                   lm_dtype=torch.float32, gate_init=None):
+                   lm_dtype=torch.float32, gate_init=None, neox_kw=None):
     """Random-init Flamingo through the public factory.  gate_init: None keeps the reference's zero gates
-    (helpers.py:255,258); a float f draws gates ~ U(-f, f) so the gated path is actually exercised."""
+    (helpers.py:255,258); a float f draws gates ~ U(-f, f) so the gated path is actually exercised.  neox_kw: build
+    the LM with build_neox(neox_kw) instead of an MPT from mpt_kw (pass mpt_kw=None)."""
     torch.manual_seed(seed)
     with torch.device(device):
         vit = VisionTransformer(**vit_cfg)
-    lm = build_mpt(mpt_kw, dtype=lm_dtype, device=device, seed=seed + 1)
-    base_vocab = mpt_kw["vocab_size"]
+    if neox_kw is not None:
+        lm = build_neox(neox_kw, dtype=lm_dtype, device=device, seed=seed + 1)
+        base_vocab = neox_kw["vocab_size"]
+    else:
+        lm = build_mpt(mpt_kw, dtype=lm_dtype, device=device, seed=seed + 1)
+        base_vocab = mpt_kw["vocab_size"]
     tok = SimpleTokenizer(base_vocab)
     model, image_processor, tok = create_model_and_transforms(
         CLIPVisionStandIn(vit), None, lm, tok, cross_attn_every_n_layers=cross_attn_every_n_layers,
