@@ -257,6 +257,28 @@ int ofk_rope_pack(const void* src_q, const void* src_k, const void* src_v, long 
                   const float* sin, long long cs_bstride, long long ld_cs, void* q, long long q_bstride, long long ldq,
                   int q_width, void* k, long long k_bstride, long long ldk, int k_width, void* v, long long v_bstride,
                   long long ldv, int v_width, void* stream);
+
+/* ofk_rope_append_dev: the one-token rotary packing of a captured decode step (the companion of ofk_attn_decode_dev,
+ * in place of ofk_rope_pack + ofk_kv_append).  For each batch entry b, from the interleaved row qkv + b * qkv_bstride
+ * (heads of (q | k | v), head_dim columns each) it writes
+ *   q + b * q_bstride:  the rotated q, heads * head_dim columns (unpadded);
+ *   cache + b * cache_bstride + (*pos_dev) * ld:  the rotated k in columns [0, heads * head_dim) and v in
+ *     [heads * head_dim, 2 * heads * head_dim), the KV-cache row layout;
+ *   key_mask[b * mask_bstride + *pos_dev] = (new_masked != NULL && new_masked[b] != 0), when key_mask is non-NULL.
+ * The rotation is ofk_rope_pack's, bit for bit (the same device function), with cos, sin f32 at b * cs_bstride + j
+ * (cs_bstride 0 = one table for every batch entry); rot = 0 turns it off and cos/sin may be NULL.  A position outside
+ * [0, capacity) writes q only.
+ * Requirements: qkv, q, cache, pos_dev non-NULL, batch and heads >= 1, head_dim a positive multiple of 8, rot even in
+ *   [0, head_dim], cos and sin non-NULL with cs_bstride >= 0 when rot > 0, capacity >= 1, qkv_bstride >= 3 * heads *
+ *   head_dim, q_bstride >= heads * head_dim, ld >= 2 * heads * head_dim, cache_bstride >= capacity * ld and, with a
+ *   key_mask, mask_bstride >= capacity (OFK_ERR_ARG); qkv, q and cache 16-byte aligned with their strides multiples of
+ *   8 elements, cos, sin and pos_dev 4-byte aligned (OFK_ERR_ALIGN).  Every argument is checked before the first CUDA
+ *   call. */
+int ofk_rope_append_dev(const void* qkv, long long qkv_bstride, int batch, int heads, int head_dim, int rot,
+                        const float* cos, const float* sin, long long cs_bstride, void* q, long long q_bstride,
+                        void* cache, long long cache_bstride, long long ld, int capacity, const int* pos_dev,
+                        unsigned char* key_mask, long long mask_bstride, const unsigned char* new_masked,
+                        void* stream);
 int ofk_rope_unpack_bwd(const void* dq, long long dq_bstride, long long lddq, const void* dk, long long dk_bstride,
                         long long lddk, const void* dv, long long dv_bstride, long long lddv, int width, int batch,
                         int rows, int heads, int head_dim, int rot, const float* cos, const float* sin,

@@ -72,6 +72,8 @@ _SIGNATURES = {
     "ofk_rope_pack": (c_int, [c_void_p, c_void_p, c_void_p, c_ll, c_ll, c_int, c_int, c_int, c_int, c_int, c_int,
                               c_void_p, c_void_p, c_ll, c_ll, c_void_p, c_ll, c_ll, c_int, c_void_p, c_ll, c_ll, c_int,
                               c_void_p, c_ll, c_ll, c_int, c_void_p]),
+    "ofk_rope_append_dev": (c_int, [c_void_p, c_ll, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_ll, c_void_p,
+                                    c_ll, c_void_p, c_ll, c_ll, c_int, c_void_p, c_void_p, c_ll, c_void_p, c_void_p]),
     "ofk_rope_unpack_bwd": (c_int, [c_void_p, c_ll, c_ll, c_void_p, c_ll, c_ll, c_void_p, c_ll, c_ll, c_int, c_int, c_int,
                                     c_int, c_int, c_int, c_void_p, c_void_p, c_ll, c_ll, c_void_p, c_ll, c_ll,
                                     c_void_p]),

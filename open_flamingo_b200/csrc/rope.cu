@@ -16,6 +16,10 @@
 // With rot = 0 nothing is rotated and the kernel only re-lays heads out: the cached path uses that to pad the K/V rows
 // of its cache (K columns, then V columns, head_dim per head) to the padded width.
 //
+// ofk_rope_append_dev is the one-token form for a captured decode step: it writes q unpadded and the rotated K and the
+// V into the KV-cache row at a position read on the device (and that row's key-mask byte), so that one CUDA graph
+// serves every position.  It rotates with the same device function as ofk_rope_pack, so the two agree bit for bit.
+//
 // ofk_rope_unpack_bwd is the adjoint: from the padded dq, dk, dv it writes the gradient of the interleaved rows,
 // applying the transposed rotation  dx = dy * cos + rotate_half^T(dy * sin),  rotate_half^T(u) = (u[rot/2 .. rot),
 // -u[0 .. rot/2)),  in fp32 with one bf16 rounding; the padding columns are not read.
@@ -56,6 +60,18 @@ struct UnpackParams {
   int rows, heads, hd, rot, width;
 };
 
+struct AppendParams {
+  const __nv_bfloat16* src;      // [batch, heads * 3 * hd] interleaved (q | k | v) per head
+  __nv_bfloat16* q;              // [batch, heads * hd]
+  __nv_bfloat16* cache;          // [batch, capacity, >= 2 * heads * hd]: K columns, then V columns
+  const float *cos, *sin;        // [1 or batch, rot]
+  const int* pos;
+  unsigned char* key_mask;       // [batch, >= capacity] or NULL
+  const unsigned char* new_masked;
+  long long src_bs, q_bs, cache_bs, ld, cs_bs, mask_bs;
+  int heads, hd, rot, capacity;
+};
+
 __device__ __forceinline__ float ld_bf16(const __nv_bfloat16* p) { return __bfloat162float(*p); }
 
 __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
@@ -67,6 +83,27 @@ __device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
   f[4] = bf16_lo(u.z); f[5] = bf16_hi(u.z); f[6] = bf16_lo(u.w); f[7] = bf16_hi(u.w);
 }
 
+// Columns [j0, j0 + 8) of one head x (bf16, 16-byte aligned at j0) with the first `rot` columns rotated by the
+// row's c, s: the one place where ofk_rope_pack and ofk_rope_append_dev round, so that they round alike.
+__device__ __forceinline__ uint4 rotate8(const __nv_bfloat16* x, int j0, int rot, const float* c, const float* s) {
+  uint4 out = *reinterpret_cast<const uint4*>(x + j0);
+  if (j0 < rot) {
+    const int half = rot / 2;
+    float f[8];
+    unpack8(out, f);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int j = j0 + e;
+      if (j < rot) {
+        const float partner = j < half ? -ld_bf16(x + j + half) : ld_bf16(x + j - half);
+        f[e] = __fadd_rn(__fmul_rn(f[e], c[j]), __fmul_rn(partner, s[j]));
+      }
+    }
+    out = pack8(f);   // the unrotated elements are bf16 values: packing them again is exact
+  }
+  return out;
+}
+
 // One CTA per (batch row, part); blockIdx.x = b * rows + t, blockIdx.y = part (0 q, 1 k, 2 v).
 __global__ void __launch_bounds__(THREADS) rope_pack_kernel(const PackParams p) {
   const int part = blockIdx.y;
@@ -75,7 +112,6 @@ __global__ void __launch_bounds__(THREADS) rope_pack_kernel(const PackParams p) 
   const long long b = blockIdx.x / p.rows, t = blockIdx.x % p.rows;
   const int W = p.width[part];
   const bool rotate = part < 2 && p.rot > 0;
-  const int half = p.rot / 2;
   src += b * p.src_bs + t * p.src_ld;
   __nv_bfloat16* dst = p.dst[part] + b * p.dst_bs[part] + t * p.dst_ld[part];
   const float* c = rotate ? p.cos + b * p.cs_bs + t * p.cs_ld : nullptr;
@@ -86,22 +122,38 @@ __global__ void __launch_bounds__(THREADS) rope_pack_kernel(const PackParams p) 
     uint4 out = make_uint4(0u, 0u, 0u, 0u);
     if (j0 < p.hd) {
       const __nv_bfloat16* x = src + (long long)h * p.src_hs;
-      out = *reinterpret_cast<const uint4*>(x + j0);
-      if (rotate && j0 < p.rot) {
-        float f[8];
-        unpack8(out, f);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const int j = j0 + e;
-          if (j < p.rot) {
-            const float partner = j < half ? -ld_bf16(x + j + half) : ld_bf16(x + j - half);
-            f[e] = __fadd_rn(__fmul_rn(f[e], c[j]), __fmul_rn(partner, s[j]));
-          }
-        }
-        out = pack8(f);   // the unrotated elements are bf16 values: packing them again is exact
-      }
+      out = rotate ? rotate8(x, j0, p.rot, c, s) : *reinterpret_cast<const uint4*>(x + j0);
     }
     *reinterpret_cast<uint4*>(dst + (long long)h * W + j0) = out;
+  }
+}
+
+// One CTA per (batch row, part), blockIdx.x = b, blockIdx.y = part (0 q, 1 k, 2 v).  q goes to its own row; k and v go
+// to cache row *pos of their batch entry (K columns, then V columns), and nowhere when *pos is outside [0, capacity).
+// The k CTA also writes the row's key-mask byte, as ofk_kv_append does.
+__global__ void __launch_bounds__(THREADS) rope_append_dev_kernel(const AppendParams p) {
+  const int part = blockIdx.y;
+  const long long b = blockIdx.x;
+  const int D = p.heads * p.hd;
+  __nv_bfloat16* dst;
+  if (part == 0) {
+    dst = p.q + b * p.q_bs;
+  } else {
+    const int pos = *p.pos;
+    if (pos < 0 || pos >= p.capacity) return;
+    dst = p.cache + b * p.cache_bs + pos * p.ld + (part - 1) * D;
+    if (part == 1 && p.key_mask != nullptr && threadIdx.x == 0)
+      p.key_mask[b * p.mask_bs + pos] = (p.new_masked != nullptr && p.new_masked[b] != 0) ? 1 : 0;
+  }
+  const __nv_bfloat16* src = p.src + b * p.src_bs + part * p.hd;
+  const bool rotate = part < 2 && p.rot > 0;
+  const float* c = rotate ? p.cos + b * p.cs_bs : nullptr;
+  const float* s = rotate ? p.sin + b * p.cs_bs : nullptr;
+  for (int i = threadIdx.x; i < D / 8; i += THREADS) {
+    const int h = i * 8 / p.hd, j0 = i * 8 % p.hd;
+    const __nv_bfloat16* x = src + (long long)h * 3 * p.hd;
+    *reinterpret_cast<uint4*>(dst + h * p.hd + j0) =
+        rotate ? rotate8(x, j0, p.rot, c, s) : *reinterpret_cast<const uint4*>(x + j0);
   }
 }
 
@@ -201,6 +253,34 @@ extern "C" int ofk_rope_pack(const void* src_q, const void* src_k, const void* s
   p.cos = cos; p.sin = sin; p.cs_bs = cs_bstride; p.cs_ld = ld_cs;
   p.rows = rows; p.heads = heads; p.hd = head_dim; p.rot = rot;
   rope_pack_kernel<<<dim3((unsigned)((long long)batch * rows), 3), THREADS, 0, (cudaStream_t)stream>>>(p);
+  OFK_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int ofk_rope_append_dev(const void* qkv, long long qkv_bstride, int batch, int heads, int head_dim, int rot,
+                                   const float* cos, const float* sin, long long cs_bstride, void* q,
+                                   long long q_bstride, void* cache, long long cache_bstride, long long ld, int capacity,
+                                   const int* pos_dev, unsigned char* key_mask, long long mask_bstride,
+                                   const unsigned char* new_masked, void* stream) {
+  if (!qkv || !q || !cache || !pos_dev) return ofk_set_error(OFK_ERR_ARG, "rope_append_dev: null pointer");
+  int rc = check_common(batch, 1, heads, head_dim, rot, cos, sin, cs_bstride, rot);
+  if (rc != 0) return rc;
+  if (capacity < 1) return ofk_set_error(OFK_ERR_ARG, "rope_append_dev: capacity must be >= 1");
+  const long long D = (long long)heads * head_dim;
+  if (qkv_bstride < 3 * D || q_bstride < D || ld < 2 * D || cache_bstride < capacity * ld ||
+      (key_mask != nullptr && mask_bstride < capacity))
+    return ofk_set_error(OFK_ERR_ARG, "rope_append_dev: a stride is below its row width");
+  if (misaligned(qkv, 16) || misaligned(q, 16) || misaligned(cache, 16) || misaligned(pos_dev, 4))
+    return ofk_set_error(OFK_ERR_ALIGN, "rope_append_dev: qkv, q and cache must be 16-byte aligned, pos_dev 4-byte");
+  if ((qkv_bstride | q_bstride | cache_bstride | ld) % 8 != 0)
+    return ofk_set_error(OFK_ERR_ALIGN, "rope_append_dev: strides must be multiples of 8 elements");
+  AppendParams p{};
+  p.src = (const __nv_bfloat16*)qkv; p.q = (__nv_bfloat16*)q; p.cache = (__nv_bfloat16*)cache;
+  p.cos = cos; p.sin = sin; p.pos = pos_dev; p.key_mask = key_mask; p.new_masked = new_masked;
+  p.src_bs = qkv_bstride; p.q_bs = q_bstride; p.cache_bs = cache_bstride; p.ld = ld; p.cs_bs = cs_bstride;
+  p.mask_bs = mask_bstride;
+  p.heads = heads; p.hd = head_dim; p.rot = rot; p.capacity = capacity;
+  rope_append_dev_kernel<<<dim3((unsigned)batch, 3), THREADS, 0, (cudaStream_t)stream>>>(p);
   OFK_CHECK_LAUNCH();
   return 0;
 }

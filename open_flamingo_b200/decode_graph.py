@@ -2,25 +2,31 @@
 
 An eager decode step of OF-3B issues about 24 x 40 kernel launches through Python and ctypes, and the GPU waits on that
 host work.  With a fixed-capacity kv_cache.KVCache nothing in a one-token step varies on the host: the new token's cache
-row and the key count live in a device int32 pair (ops.kv_append and ops.attn_decode_dev read them), the cache buffers
-never move, and the padding of the keys is a byte buffer beside them.  So the step is captured once per shape key
-(batch, capacity, media shape, device) and replayed:
+row and the key count live in a device int32 pair (ops.kv_append, ops.rope_append_dev and ops.attn_decode_dev read
+them), the cache buffers never move, and the padding of the keys is a byte buffer beside them.  So the step is captured
+once per shape key (batch, capacity, media shape, device) and replayed.  Two LM families are served:
 
-    wte(ids) -> per FlamingoLayer: gated block (fused.GatedXattnBlockFn on static media K/V and text_time), then
-    FastMptBlock.decode_step -> norm_f -> lm_head
+  MPT (OF-3B, OF-9B):   wte(ids) -> per FlamingoLayer: gated block (fused.GatedXattnBlockFn on static media K/V and
+                        text_time), then FastMptBlock.decode_step -> norm_f -> lm_head
+  GPT-NeoX (OF-4B):     embed_in(ids) -> rotary_emb(h, positions) -> per FlamingoLayer: gated block, then
+                        FastNeoXBlock.decode_step -> final_layer_norm -> embed_out
 
-HF's own `wte`, `norm_f` and `lm_head` run under the caller's autocast (with autocast's weight cache off, so the graph
-never reads a cast that is freed when the autocast region ends).  MptModel.forward is bypassed: its per-call mask and
-ALiBi construction are not capturable, and the decoder blocks take their slopes and key mask from elsewhere anyway.
+HF's own embedding, rotary module, final norm and output head run under the caller's autocast (with autocast's weight
+cache off, so the graph never reads a cast that is freed when the autocast region ends).  MptModel.forward and
+GPTNeoXModel.forward are bypassed: their per-call mask construction (and MPT's ALiBi) are not capturable, and the
+decoder blocks take their slopes and key mask from elsewhere anyway.  GPT-NeoX's rotary tables come from HF's module run
+inside the graph on a static int64 position buffer holding the cache length, the position_ids GPTNeoXModel makes when
+the caller passes none: the same torch ops on the same values give the eager step's cos and sin.
 
-Everything the graph reads is a static buffer: ids, the position pair, the new token's padding byte, the media K/V of
-every gated layer, text_time, the cache rows and the key mask.  A cache is bound to a graph by moving its rows into
-the graph's cache buffers (its first replay in a call); the media inputs are refreshed at the same time, so one
-capture serves every later call with the same key.  A call is a run of consecutive replayed steps on one cache: a
-step on another cache or media, or after an eager step, a crop or a reset of the cache, starts a new one.  Every
-parameter the graph reads is snapshotted as (data_ptr, _version) at capture and checked at the start of each call; a
-change (load_state_dict, an optimizer step) re-captures.  A capture that fails leaves that key on the eager path and
-keeps the error in `DecodeGraphs.error`.  The replayed step computes what the eager cached step computes, bit for bit.
+Everything the graph reads is a static buffer: ids, the position pair (and GPT-NeoX's position_ids), the new token's
+padding byte, the media K/V of every gated layer, text_time, the cache rows and the key mask.  A cache is bound to a
+graph by moving its rows into the graph's cache buffers (its first replay in a call); the media inputs are refreshed at
+the same time, so one capture serves every later call with the same key.  A call is a run of consecutive replayed steps
+on one cache: a step on another cache or media, or after an eager step, a crop or a reset of the cache, starts a new
+one.  Every parameter the graph reads is snapshotted as (data_ptr, _version) at capture and checked at the start of
+each call; a change (load_state_dict, an optimizer step) re-captures.  A capture that fails leaves that key on the eager
+path and keeps the error in `DecodeGraphs.error`.  The replayed step computes what the eager cached step computes, bit
+for bit.
 
 The shape key also holds whether inference mode is on: tensors made under `torch.inference_mode` cannot be updated in
 place outside it, so a graph whose buffers were made there is never fed under `torch.no_grad`, nor the reverse.
@@ -62,8 +68,36 @@ def _autocast_bf16():
     return torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == torch.bfloat16
 
 
+def _is_neox(lm):
+    """A GPT-NeoX LM (HF GPTNeoXForCausalLM); otherwise the LM is taken for an MPT."""
+    return hasattr(lm, "gpt_neox")
+
+
+def _heads(fast):
+    """(heads, head_dim) of a decoder block's attention."""
+    if isinstance(fast, lm_blocks.FastNeoXBlock):
+        a = fast.block.attention
+        return a.config.num_attention_heads, a.head_size
+    a = fast.block.attn
+    return a.n_heads, a.head_dim
+
+
+def _neox_model_supported(lm):
+    """The GPT-NeoX model parts around the blocks are ones the graph replays as GPTNeoXModel.forward runs them: HF's
+    default rotary embedding (other rope types, such as dynamic scaling, update their tables from host-side lengths) and
+    an embedding dropout that is off."""
+    m = lm.gpt_neox
+    if not hasattr(lm, "embed_out") or not all(hasattr(m, n) for n in ("embed_in", "rotary_emb", "final_layer_norm")):
+        return False
+    if getattr(m.rotary_emb, "rope_type", None) != "default":
+        return False
+    drop = getattr(m, "emb_dropout", None)
+    return drop is None or not (drop.training and drop.p > 0)
+
+
 def eligible(lm, input_ids, attention_mask, cache, use_cached_media, kwargs):
-    """True when this forward is a one-token step the graph computes exactly as the eager cached path would."""
+    """True when this forward is a one-token step the graph computes exactly as the eager cached path would.  A
+    position_ids keyword (which `generate` does not pass to a Flamingo LM) is one of the calls declined."""
     if not (isinstance(cache, KVCache) and cache.capacity is not None and cache.key_mask_known):
         return False
     if not input_ids.is_cuda or input_ids.dim() != 2 or input_ids.shape[1] != 1 or not use_cached_media:
@@ -84,20 +118,35 @@ def eligible(lm, input_ids, attention_mask, cache, use_cached_media, kwargs):
         return False
     if cache.key_mask is None or cache.key_mask.shape[0] != B or cache.key_mask.device != input_ids.device:
         return False
-    if not all(hasattr(lm, n) for n in ("transformer", "lm_head")) or not hasattr(lm.transformer, "norm_f"):
+    neox = _is_neox(lm)
+    if neox:
+        if not _neox_model_supported(lm):
+            return False
+    elif not all(hasattr(lm, n) for n in ("transformer", "lm_head")) or not hasattr(lm.transformer, "norm_f"):
         return False
     layers = lm._get_decoder_layers()
     if len(layers) != len(cache.layers):
         return False
     for layer, cl in zip(layers, cache.layers):
         fast = getattr(layer, "_fast_block", None)
-        if fast is None or not fast.supported(input_ids, fast.slopes(input_ids.device), False):
+        if fast is None:
             return False
-        a = fast.block.attn
+        if neox:
+            # the rotary tables are checked by the capture, once HF's module has made them
+            if not isinstance(fast, lm_blocks.FastNeoXBlock) or not fast.block_supported(
+                    input_ids, fast.records_outputs(kwargs.get("output_attentions"),
+                                                    kwargs.get("output_hidden_states"))):
+                return False
+            a = fast.block.attention
+        else:
+            if not fast.supported(input_ids, fast.slopes(input_ids.device), False):
+                return False
+            a = fast.block.attn
+        heads, hd = _heads(fast)
         if a.layer_idx is None or cache.layers[a.layer_idx] is not cl:
             return False
         if not cl.is_initialized or cl.length != past or cl.buf.dtype != torch.bfloat16 or cl.buf.shape[0] != B or \
-                cl.buf.device != input_ids.device or cl.heads != a.n_heads or cl.head_dim != a.head_dim:
+                cl.buf.device != input_ids.device or cl.heads != heads or cl.head_dim != hd:
             return False
         if layer.gated_cross_attn_layer is not None:
             if layer.vis_x is None or layer.media_locations is None or layer.vis_x.dim() != 4 or \
@@ -146,8 +195,10 @@ class _Entry:
         self.text_time = torch.zeros((B, 1), device=device, dtype=torch.int32)
         self.gated = [None if layer.gated_cross_attn_layer is None else
                       _Gated(layer.gated_cross_attn_layer, B, T_img, n, device) for layer in layers]
-        a = layers[0]._fast_block.block.attn
-        self.workspace = ops.decode_workspace(device, B, a.n_heads, a.head_dim, cache.capacity)
+        # GPT-NeoX: the position_ids GPTNeoXModel.forward makes for the step, [1, 1] int64 = the cache length
+        self.positions = torch.zeros((1, 1), device=device, dtype=torch.int64) if _is_neox(lm) else None
+        heads, hd = _heads(layers[0]._fast_block)
+        self.workspace = ops.decode_workspace(device, B, heads, hd, cache.capacity)
         self.graph = None
         self.logits = None
         self.failed = False
@@ -205,6 +256,8 @@ class _Entry:
         self.ids.copy_(input_ids)
         self.pos_nk[0:1].fill_(past)
         self.pos_nk[1:2].fill_(past + 1)
+        if self.positions is not None:
+            self.positions.fill_(past)
         if attention_mask is None:
             self.new_masked.zero_()
         else:
@@ -212,9 +265,14 @@ class _Entry:
 
 
 def _params(lm):
-    """Every parameter a decode step reads."""
-    ps = list(lm.transformer.wte.parameters()) + list(lm.transformer.norm_f.parameters()) + \
-        list(lm.lm_head.parameters())
+    """Every parameter a decode step reads (GPT-NeoX: and the rotary module's frequencies)."""
+    if _is_neox(lm):
+        m = lm.gpt_neox
+        ps = list(m.embed_in.parameters()) + list(m.final_layer_norm.parameters()) + list(lm.embed_out.parameters()) + \
+            [m.rotary_emb.inv_freq]
+    else:
+        ps = list(lm.transformer.wte.parameters()) + list(lm.transformer.norm_f.parameters()) + \
+            list(lm.lm_head.parameters())
     for layer in lm._get_decoder_layers():
         if layer.gated_cross_attn_layer is not None:
             ps += list(layer.gated_cross_attn_layer.parameters())
@@ -225,12 +283,15 @@ def _params(lm):
 def _kernel_weights(lm):
     """The parameters whose bf16 copies (fused.w16) the graph reads."""
     ws = []
+    # the weights() positions of the GEMM weights: GPT-NeoX query_key_value, dense, dense_h_to_4h, dense_4h_to_h; MPT
+    # Wqkv, out_proj, up_proj, down_proj
+    gemm = (2, 4, 8, 10) if _is_neox(lm) else (1, 2, 4, 5)
     for layer in lm._get_decoder_layers():
         x = layer.gated_cross_attn_layer
         if x is not None:
             ws += [x.attn.to_q.weight, x.attn.to_out.weight, x.ff[1].weight, x.ff[3].weight]
         w = layer._fast_block.weights()
-        ws += [w[1], w[2], w[4], w[5]]
+        ws += [w[i] for i in gemm]
     return ws
 
 
@@ -256,8 +317,18 @@ class DecodeGraphs:
     def _body(self, lm, e, cache):
         layers = lm._get_decoder_layers()
         # autocast's weight-cast cache lives until the caller's autocast region ends; a graph must not read from it
+        neox = _is_neox(lm)
         with torch.autocast("cuda", dtype=torch.bfloat16, cache_enabled=False):
-            h = lm.transformer.wte(e.ids)
+            if neox:
+                m = lm.gpt_neox
+                h = m.embed_in(e.ids)
+                # GPTNeoXModel.forward's rotary tables, from HF's module on the step's position_ids
+                pe = (m.rotary_emb(h, e.positions),)
+                if not all(layer._fast_block.supported(h, pe[0], False) for layer in layers):
+                    raise ValueError("decode graph: the GPT-NeoX blocks do not take these rotary tables")
+            else:
+                h = lm.transformer.wte(e.ids)
+                pe = ()
             for layer, g, cl in zip(layers, e.gated, cache.layers):
                 if g is not None:
                     x = g.xattn
@@ -266,7 +337,9 @@ class DecodeGraphs:
                         h.float(), g.media_shape, g.media_shape, e.text_time, g.mode, a.heads, g.n, a.norm.weight,
                         a.norm.bias, a.to_q.weight, a.to_kv.weight, a.to_out.weight, x.attn_gate, x.ff[0].weight,
                         x.ff[0].bias, x.ff[1].weight, x.ff[3].weight, x.ff_gate, g.kv_cache())
-                h = layer._fast_block.decode_step(h.float(), cl, e.pos_nk, e.key_mask, e.new_masked, e.workspace)
+                h = layer._fast_block.decode_step(h.float(), cl, e.pos_nk, e.key_mask, e.new_masked, e.workspace, *pe)
+            if neox:
+                return lm.embed_out(m.final_layer_norm(h))
             return lm.lm_head(lm.transformer.norm_f(h))
 
     def _capture(self, lm, e, cache):
@@ -277,14 +350,16 @@ class DecodeGraphs:
         s.wait_stream(cur)
         # one eager step on the capture stream first: kernel attributes, tensor maps, the w16 copies, the slopes and
         # every lazily made buffer come into being outside the capture.  It computes this very step, so it is harmless.
+        # It also raises, before any capture, for rotary tables the GPT-NeoX blocks do not take.
         with torch.cuda.stream(s):
             self._body(lm, e, cache)
         cur.wait_stream(s)
         params = _params(lm)
         e.snapshot = _snapshot(params)
-        # the graph holds no reference to memory made outside it: keep the weight copies and slopes it reads alive
-        e.keep = tuple(fused.w16(p) for p in _kernel_weights(lm)) + \
-            tuple(layer._fast_block.slopes(e.ids.device) for layer in lm._get_decoder_layers())
+        # the graph holds no reference to memory made outside it: keep the weight copies and (MPT) slopes it reads alive
+        e.keep = tuple(fused.w16(p) for p in _kernel_weights(lm))
+        if not _is_neox(lm):
+            e.keep += tuple(layer._fast_block.slopes(e.ids.device) for layer in lm._get_decoder_layers())
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph, stream=s):
             e.logits = self._body(lm, e, cache)

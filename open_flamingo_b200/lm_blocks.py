@@ -325,7 +325,8 @@ class FastMptBlock:
 # layout, zero columns add exact zeros to q k^T, to P v and to every backward product, so the result is the head_dim-80
 # attention.  The attention output then has H * 128 columns; the out-projection reads it through a copy of Wd with the
 # same zero columns (_padded_w16), and in the backward the dgrad GEMM with that copy yields the padded d_o directly.
-# Decoding one token runs the decode kernel at head_dim 80 directly, on an unpadded KV cache.
+# Decoding one token runs the decode kernel at head_dim 80 directly, on an unpadded KV cache; its graph-captured form
+# (decode_step_neox_block_forward) writes the new K/V row with ops.rope_append_dev at a position read on the device.
 
 
 def _neox_width(hd):
@@ -475,6 +476,27 @@ def cached_neox_block_forward(x, layer, mask, pure_flag, cos, sin, heads, parall
                       w1, b1, w2, b2, keep_z=False)[0].view(B, nq, D)
 
 
+def decode_step_neox_block_forward(x, layer, pos_nk, key_mask, new_masked, workspace, cos, sin, heads, parallel, eps1,
+                                   eps2, n1_w, n1_b, wqkv, bqkv, wd, bd, n2_w, n2_b, w1, b1, w2, b2):
+    """cached_neox_block_forward for one new token with its position on the device, so that the step can be captured
+    in a CUDA graph once and replayed at every position (the GPT-NeoX decode_step_block_forward).  pos_nk, key_mask,
+    new_masked, workspace: as there; cos, sin: f32 [1 or B, 1, rot] of the new token's position.  The GEMMs, epilogues
+    and shapes are the eager nq == 1 path's, and ops.rope_append_dev rotates as ops.rope_pack does while writing K and V
+    into cache row pos_nk[0], so the result is the eager path's, bit for bit.  x: [B, 1, D] f32; returns the same."""
+    B, _, D = x.shape
+    hd = D // heads
+    x2d = _rows(x)
+    xn, _, _ = ops.layernorm_fwd(x2d, n1_w, n1_b, eps1, want_stats=False)
+    qkv = ops.gemm(xn, w16(wqkv), epi=L.EPI_BIAS_BF16, bias=bqkv)                   # [B, 3D]
+    del xn
+    buf = layer.buf
+    q = ops.rope_append_dev(qkv, heads, hd, cos, sin, buf, pos_nk[0:1], key_mask=key_mask, new_masked=new_masked)
+    del qkv
+    o = ops.attn_decode_dev(q, buf[..., :D], buf[..., D:], heads, hd, float(hd ** -0.5), pos_nk[1:2],
+                            key_mask=key_mask, workspace=workspace)
+    return _neox_tail(x2d, o, parallel, eps2, w16(wd), bd, n2_w, n2_b, w1, b1, w2, b2, keep_z=False)[0].view(B, 1, D)
+
+
 class FastNeoXBlock:
     """Callable with HF GPTNeoXLayer.forward's signature; returns None when the fast path does not apply, and the
     block's output tensor otherwise."""
@@ -497,16 +519,24 @@ class FastNeoXBlock:
     def supported(self, hidden_states, position_embeddings, record_outputs):
         """The block and call are ones the kernels evaluate, whatever the cache.  record_outputs: see
         records_outputs."""
-        b = self.block
-        a = b.attention
-        if not ENABLED or not hidden_states.is_cuda or record_outputs or position_embeddings is None:
+        if position_embeddings is None or not self.block_supported(hidden_states, record_outputs):
             return False
         cos, sin = position_embeddings
+        if cos.dtype != f32 or sin.dtype != f32 or cos.dim() != 3 or cos.shape != sin.shape or \
+                cos.stride() != sin.stride() or cos.stride(2) != 1 or cos.shape[2] % 2 or \
+                not 0 < cos.shape[2] <= self.block.attention.head_size:
+            return False
+        return True
+
+    def block_supported(self, hidden_states, record_outputs):
+        """The part of `supported` that does not read the rotary tables: what decode_graph can check before the model's
+        rotary module has run."""
+        b = self.block
+        a = b.attention
+        if not ENABLED or not hidden_states.is_cuda or record_outputs:
+            return False
         hd = a.head_size
         if hd not in (64, 80, 128) or abs(a.scaling - hd ** -0.5) > 1e-9:
-            return False
-        if cos.dtype != f32 or sin.dtype != f32 or cos.dim() != 3 or cos.shape != sin.shape or \
-                cos.stride() != sin.stride() or cos.stride(2) != 1 or cos.shape[2] % 2 or not 0 < cos.shape[2] <= hd:
             return False
         if b.training and (a.attention_dropout > 0 or b.post_attention_dropout.p > 0 or b.post_mlp_dropout.p > 0):
             return False
@@ -527,6 +557,20 @@ class FastNeoXBlock:
                 a.dense.weight, a.dense.bias, b.post_attention_layernorm.weight, b.post_attention_layernorm.bias,
                 b.mlp.dense_h_to_4h.weight, b.mlp.dense_h_to_4h.bias, b.mlp.dense_4h_to_h.weight,
                 b.mlp.dense_4h_to_h.bias)
+
+    def step_args(self):
+        """The head count, residual form and LayerNorm eps of the block, then its weights: the arguments after cos and
+        sin of cached_neox_block_forward and decode_step_neox_block_forward."""
+        b = self.block
+        return (b.attention.config.num_attention_heads, bool(b.use_parallel_residual), b.input_layernorm.eps,
+                b.post_attention_layernorm.eps) + self.weights()
+
+    def decode_step(self, x, layer, pos_nk, key_mask, new_masked, workspace, position_embeddings):
+        """One captured decode step of this block (decode_step_neox_block_forward); position_embeddings: the (cos, sin)
+        of the new token's position."""
+        cos, sin = position_embeddings
+        return decode_step_neox_block_forward(x, layer, pos_nk, key_mask, new_masked, workspace, cos, sin,
+                                              *self.step_args())
 
     def applicable(self, hidden_states, position_embeddings, layer_past, use_cache, record_outputs):
         """The uncached path (FrozenNeoXBlockFn, forward and backward)."""
@@ -561,7 +605,6 @@ class FastNeoXBlock:
                 return None
         elif not self.applicable(hidden_states, position_embeddings, layer_past, use_cache, record):
             return None
-        b = self.block
         B, T, _ = hidden_states.shape
         cos, sin = position_embeddings
         if cos.shape[0] not in (1, B) or cos.shape[1] != T:
@@ -574,8 +617,7 @@ class FastNeoXBlock:
                 return None
         x = hidden_states if hidden_states.dtype == f32 else hidden_states.float()
         flag = pure_causal_flag if mask is not None else None
-        rest = (cos, sin, b.attention.config.num_attention_heads, bool(b.use_parallel_residual), b.input_layernorm.eps,
-                b.post_attention_layernorm.eps) + self.weights()
+        rest = (cos, sin) + self.step_args()
         if layer is not None:
             out = cached_neox_block_forward(x, layer, mask, flag, *rest)
         else:

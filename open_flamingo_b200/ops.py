@@ -677,6 +677,49 @@ def rope_pack(src, heads, head_dim, cos=None, sin=None, *, q=None, k=None, v=Non
     return outs[0][0], outs[1][0], outs[2][0]
 
 
+def rope_append_dev(qkv, heads, head_dim, cos, sin, cache, pos_dev, *, key_mask=None, new_masked=None, q=None):
+    """The one-token rope_pack of a captured decode step (ofk_rope_append_dev): rotates q and k of the interleaved
+    query_key_value rows qkv [B, heads * 3 * head_dim] (bf16, unit inner stride) with cos/sin fp32 [1 or B, 1, rot]
+    (None: no rotation), writes q to `q` [B, heads * head_dim] (allocated when None) and the rotated K and the V into
+    row pos = pos_dev[0] of `cache` [B, capacity, 2 * heads * head_dim] (K columns, then V), and sets
+    key_mask[b, pos] = new_masked[b] != 0 as kv_append does.  Nothing but q is written for a pos outside
+    [0, capacity).  key_mask: 1-byte [B, >= capacity], unit inner stride; new_masked: 1-byte [B]; pos_dev: int32 CUDA
+    tensor.  Returns q."""
+    L.require_cuda(qkv, cos, sin, cache, pos_dev, key_mask, new_masked, q)
+    D = heads * head_dim
+    if qkv.dtype != bf16 or qkv.dim() != 2 or qkv.shape[1] != 3 * D or qkv.stride(1) != 1:
+        raise ValueError(f"qkv must be a bf16 [B, {3 * D}] view with unit inner stride, got {tuple(qkv.shape)} "
+                         f"{qkv.dtype}")
+    B = qkv.shape[0]
+    if cache.dtype != bf16 or cache.dim() != 3 or cache.shape[0] != B or cache.shape[2] != 2 * D or \
+            cache.stride(2) != 1:
+        raise ValueError(f"cache must be a bf16 [{B}, capacity, {2 * D}] view with unit inner stride, got "
+                         f"{tuple(cache.shape)} {cache.dtype}")
+    cap = cache.shape[1]
+    rot = cs_bs = 0
+    if cos is not None:
+        rot = cos.shape[-1]
+        cs_bs, _ = _rope_tables(cos, sin, B, 1, rot)
+    if key_mask is not None and (key_mask.dim() != 2 or key_mask.shape[0] != B or key_mask.shape[1] < cap or
+                                 key_mask.element_size() != 1 or key_mask.stride(1) != 1):
+        raise ValueError(f"key_mask must be a 1-byte [B, >= {cap}] tensor with unit inner stride")
+    if new_masked is not None and (new_masked.numel() != B or new_masked.element_size() != 1 or
+                                   not new_masked.is_contiguous()):
+        raise ValueError(f"new_masked must be a contiguous 1-byte tensor of {B} elements")
+    if pos_dev.dtype != torch.int32 or pos_dev.numel() < 1:
+        raise ValueError("pos_dev must be an int32 device tensor")
+    if q is None:
+        q = torch.empty((B, D), device=qkv.device, dtype=bf16)
+    elif q.dtype != bf16 or q.dim() != 2 or tuple(q.shape) != (B, D) or q.stride(1) != 1:
+        raise ValueError(f"q must be a bf16 [{B}, {D}] tensor with unit inner stride")
+    L.check(L.lib().ofk_rope_append_dev(qkv.data_ptr(), qkv.stride(0), B, heads, head_dim, rot, L.ptr(cos), L.ptr(sin),
+                                        cs_bs, q.data_ptr(), q.stride(0), cache.data_ptr(), cache.stride(0),
+                                        cache.stride(1), cap, pos_dev.data_ptr(), L.ptr(key_mask),
+                                        0 if key_mask is None else key_mask.stride(0), L.ptr(new_masked),
+                                        L.stream_ptr()))
+    return q
+
+
 def rope_unpack_bwd(dq, dk, dv, heads, head_dim, cos=None, sin=None, *, out=None):
     """Adjoint of rope_pack (ofk_rope_unpack_bwd): dq/dk/dv [B, T, heads * W] bf16 views -> the gradient of the
     interleaved rows, [B, T, heads * 3 * head_dim] bf16 (`out`, allocated when None)."""

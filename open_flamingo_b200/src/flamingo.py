@@ -79,7 +79,7 @@ class Flamingo(nn.Module):
     def generate(self, vision_x: torch.Tensor, lang_x: torch.Tensor, attention_mask: torch.Tensor = None, **kwargs):
         """HF generate() conditioned on images; kwargs are forwarded (max_new_tokens, num_beams, ...).
         Returns lang_x with the generated tokens appended.  When generation uses a cache (`use_cache=True`) under
-        bf16 autocast, the frozen MPT blocks decode on the kernels through a kv_cache.KVCache (see
+        bf16 autocast, the frozen MPT and GPT-NeoX blocks decode on the kernels through a kv_cache.KVCache (see
         FlamingoLMMixin.make_kv_cache).  `cache_implementation="static"` (HF's name for a fixed-capacity cache)
         makes that cache fixed-capacity -- prompt plus new tokens, for every beam -- and replays one captured CUDA graph
         per generated token (decode_graph); where the kernels' cache is not made, the argument goes to HF."""

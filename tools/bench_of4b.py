@@ -6,8 +6,11 @@ Measures, in one process on one GPU (random-init weights at the released dims; b
   train  tokens/s of the training step (autocast bf16 forward + backward + FlatTrainer.step), frozen LM blocks on the
          kernels (lm_blocks.FrozenNeoXBlockFn) vs lm_blocks.ENABLED = False (HF's GPTNeoXLayer in eager PyTorch),
          timed in alternating rounds so that both see the same clocks;
-  decode ms per generated token of Flamingo.generate (greedy, B = 1, and 3 beams over B = 8) under autocast, kernels
-         (KVCache, ops.attn_decode at head_dim 80) vs HF (DynamicCache, sdpa), also alternating.
+  decode ms per generated token of Flamingo.generate (greedy, B = 1, and 3 beams over B = 8) under autocast, in three
+         alternating arms: kernels (KVCache, eager steps, ops.attn_decode at head_dim 80), graph
+         (cache_implementation="static": one CUDA graph replay per token, decode_graph) and HF (DynamicCache, sdpa).
+         For the graph arm also the GPU time of one replayed step between CUDA events, the capture time, and whether
+         its tokens equal the kernels arm's.
 Prints one JSON line with the card's name and power limit (nvidia-smi), as bench.py records them; --out writes it there
 too.  The training batch is (batch, 2 images, t_txt tokens); if it does not fit, pass a smaller --batch.
 """
@@ -57,12 +60,11 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--gen-tokens", type=int, default=16)
     ap.add_argument("--layers", type=int, default=None, help="LM depth (default: the released 32)")
+    ap.add_argument("--decode-only", action="store_true", help="skip the training measurement")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
 
-    from open_flamingo_b200 import lm_blocks
-    from open_flamingo_b200.testing import NEOX_3B, build_flamingo, synthetic_batch
-    from open_flamingo_b200.train import FlatTrainer
+    from open_flamingo_b200.testing import NEOX_3B, build_flamingo
     assert torch.cuda.is_available(), "bench_of4b measures on a GPU"
     torch.cuda.set_device(0)
     neox = dict(NEOX_3B)
@@ -75,7 +77,21 @@ def main():
     res = dict(model="of4b", gpu=gpu_identity(), lm_layers=neox["num_hidden_layers"], batch=args.batch,
                t_img=args.t_img, t_txt=args.t_txt)
 
-    # ---- training step
+    if not args.decode_only:
+        train(args, model, media_id, eoc_id, neox, res)
+    decode(args, model, media_id, res)
+    line = json.dumps(res)
+    print(line)
+    if args.out:
+        os.makedirs(args.out, exist_ok=True)
+        with open(os.path.join(args.out, "bench_of4b.json"), "w") as f:
+            f.write(line + "\n")
+
+
+def train(args, model, media_id, eoc_id, neox, res):
+    from open_flamingo_b200 import lm_blocks
+    from open_flamingo_b200.testing import synthetic_batch
+    from open_flamingo_b200.train import FlatTrainer
     model.train()
     trainer = FlatTrainer(model, lr=1e-4, weight_decay=0.1, max_grad_norm=1.0)
     b = synthetic_batch(args.batch, args.t_img, args.t_txt, media_id, eoc_id, neox["vocab_size"],
@@ -106,10 +122,24 @@ def main():
     res["train_step_ms_hf_lm"] = [round(t * 1e3, 2) for t in times[False]]
     res["peak_mem_gb"] = round(torch.cuda.max_memory_allocated() / 2 ** 30, 2)
     del trainer
-    model.eval()
     torch.cuda.empty_cache()
 
-    # ---- decoding
+
+def decode(args, model, media_id, res):
+    from open_flamingo_b200 import lm_blocks
+    model.eval()
+    graphs = model.lang_encoder.decode_graphs
+    capture_s = []
+    capture = graphs._capture
+
+    def timed_capture(*a, **k):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        capture(*a, **k)
+        torch.cuda.synchronize()
+        capture_s.append(time.perf_counter() - t0)
+    graphs._capture = timed_capture
+    arms = {"kernels": (True, False), "graph": (True, True), "hf": (False, False)}   # (lm_blocks.ENABLED, static)
     g = torch.Generator().manual_seed(3)
     prompt = 32
     for name, B, beams in (("greedy_b1", 1, 1), ("beam3_b8", 8, 3)):
@@ -118,30 +148,47 @@ def main():
         lang_x[:, 0] = media_id
         lang_x = lang_x.cuda()
 
-        def gen(n):
-            with torch.inference_mode(), torch.autocast("cuda", dtype=torch.bfloat16):
-                model.generate(vision_x=vision_x, lang_x=lang_x, attention_mask=torch.ones_like(lang_x),
-                               max_new_tokens=n, min_new_tokens=n, num_beams=beams, use_cache=True, pad_token_id=0,
-                               eos_token_id=None)
-        per = {True: [], False: []}
-        for on in (True, False):
+        def gen(arm, n):
+            on, static = arms[arm]
             lm_blocks.ENABLED = on
-            timed(lambda: gen(2), 1)
+            kw = dict(cache_implementation="static") if static else {}
+            with torch.inference_mode(), torch.autocast("cuda", dtype=torch.bfloat16):
+                return model.generate(vision_x=vision_x, lang_x=lang_x, attention_mask=torch.ones_like(lang_x),
+                                      max_new_tokens=n, min_new_tokens=n, num_beams=beams, use_cache=True,
+                                      pad_token_id=0, eos_token_id=None, **kw)
+        # every arm is warmed up at both lengths: the graph arm captures once per cache capacity (prompt + n rows,
+        # bucketed), and both lengths below share one bucket
+        n0 = len(capture_s)
+        for arm in arms:
+            timed(lambda: gen(arm, 2), 1)
+            timed(lambda: gen(arm, args.gen_tokens + 1), 1)
+        res[f"decode_graph_capture_ms_{name}"] = [round(t * 1e3, 1) for t in capture_s[n0:]]
+        r0 = graphs.replays
+        per = {arm: [] for arm in arms}
         for _ in range(args.rounds):
-            for on in (True, False):
-                lm_blocks.ENABLED = on
+            for arm in arms:
                 # per-token time: the difference of two lengths cancels the prompt and the vision encoder
-                t_long, t_short = timed(lambda: gen(args.gen_tokens + 1), 1), timed(lambda: gen(1), 1)
-                per[on].append((t_long - t_short) / args.gen_tokens)
-        lm_blocks.ENABLED = True
-        res[f"decode_ms_per_token_{name}_kernels"] = round(min(per[True]) * 1e3, 3)
-        res[f"decode_ms_per_token_{name}_hf"] = round(min(per[False]) * 1e3, 3)
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "bench_of4b.json"), "w") as f:
-            f.write(line + "\n")
+                t_long, t_short = timed(lambda: gen(arm, args.gen_tokens + 1), 1), timed(lambda: gen(arm, 1), 1)
+                per[arm].append((t_long - t_short) / args.gen_tokens)
+        assert graphs.error is None and graphs.replays - r0 == args.rounds * args.gen_tokens, graphs.error
+        for arm in arms:
+            res[f"decode_ms_per_token_{name}_{arm}"] = round(min(per[arm]) * 1e3, 3)
+        res[f"decode_graph_tokens_equal_kernels_{name}"] = bool(torch.equal(
+            gen("kernels", args.gen_tokens), gen("graph", args.gen_tokens)))
+        # GPU time of one replayed step: the last key's graph, replayed between events (it rewrites its last row)
+        graph = next(reversed(graphs.entries.values())).graph
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+        reps = 20
+        graph.replay()
+        ev[0].record()
+        for _ in range(reps):
+            graph.replay()
+        ev[1].record()
+        torch.cuda.synchronize()
+        res[f"decode_graph_step_gpu_ms_{name}"] = round(ev[0].elapsed_time(ev[1]) / reps, 3)
+        graphs.clear()
+    lm_blocks.ENABLED = True
+    graphs._capture = capture
 
 
 if __name__ == "__main__":
