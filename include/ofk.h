@@ -118,6 +118,27 @@ int ofk_layernorm_bwd(const void* dy, int dy_is_f32, long long lddy, int rows_pe
                       long long ldadd, float* dgamma, float* dbeta, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * RMSNorm of the LLaMA decoder blocks (HF LlamaRMSNorm), csrc/rmsnorm.cu.  One 256-thread block per row; fp32
+ * statistics summed in a fixed order, so both directions give the same bits on every launch.
+ * ofk_rmsnorm_fwd:  y(bf16) = bf16(gamma * (x * rstd)),  rstd = rsqrt(mean(x^2) + eps): LlamaRMSNorm's product order,
+ *   rounded once where autocast rounds its fp32 output as the next Linear's operand.
+ *   x: [rows, D] f32 (ldx); gamma: [D] f32; y: [rows, D] bf16 (ldy); rstd: [rows] f32 output, or NULL.
+ * ofk_rmsnorm_bwd (input gradient only: the LM's norms are frozen):
+ *   dx(f32) = rstd * (gamma * dy - xhat * mean(gamma * dy * xhat)) + dx_add,  xhat = x * rstd,
+ *   dy: [rows, D] bf16 (lddy); x, gamma, rstd: those of the forward; dx: [rows, D] f32 (lddx); dx_add: [rows, D] f32
+ *   (ldadd) or NULL, and may alias dx.
+ * Requirements: x, gamma, y (fwd) and dy, x, gamma, rstd, dx (bwd) non-NULL, rows >= 1, D a positive multiple of 8
+ *   and <= 8192, every row stride >= D (OFK_ERR_ARG); x, gamma, y, dy, dx and dx_add 16-byte aligned, rstd 4-byte,
+ *   ldx, lddx and ldadd multiples of 4 and ldy, lddy multiples of 8 (OFK_ERR_ALIGN).  Every argument is checked
+ *   before the first CUDA call.
+ */
+int ofk_rmsnorm_fwd(const float* x, long long ldx, const float* gamma, float eps, int rows, int D, void* y,
+                    long long ldy, float* rstd, void* stream);
+int ofk_rmsnorm_bwd(const void* dy, long long lddy, const float* x, long long ldx, const float* gamma,
+                    const float* rstd, int rows, int D, float* dx, long long lddx, const float* dx_add,
+                    long long ldadd, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Attention core  O = softmax(scale * Q K^T + mask) V  per (batch, head), head_dim = 64, bf16 in/out,
  * fp32 softmax, online (flash-style).  Warpgroup kernels whose QK^T / PV (and the backward's five products) are wgmma on
  * 128-byte-swizzled shared-memory tiles, P / dS fed from registers.
@@ -322,6 +343,20 @@ int ofk_gate_bwd(const float* dout, const void* branch, const float* gate, void*
  * gives the bits of a BIAS_GELU_BF16 GEMM and keeps z for the DGELU_BF16 backward (HF GPTNeoXMLP under autocast).
  * n % 8 == 0 (OFK_ERR_ARG); z and h 16-byte aligned (OFK_ERR_ALIGN). */
 int ofk_gelu_bf16(const void* z, void* h, long long n, void* stream);
+
+/* SwiGLU of the LLaMA MLP (HF LlamaMLP: act_fn(gate_proj(x)) * up_proj(x), act_fn = SiLU) on gu = [g | u]: the
+ * [rows, 2F] bf16 output (ldgu) of one GEMM against the concatenated gate|up weight, g = gu[:, :F], u = gu[:, F:].
+ * ofk_swiglu_fwd:  h(bf16) [rows, F] (ldh) = bf16(bf16(silu(g)) * u), silu(g) = g / (1 + exp(-g)) in fp32: the two
+ *   roundings autocast makes.
+ * ofk_swiglu_bwd:  from dh(bf16) [rows, F] (lddh), writes dgu(bf16) [rows, 2F] (lddgu), the operand of one dgrad GEMM
+ *   with the concatenated weight:  dgu[:, :F] = bf16(dh * u * silu'(g)) in fp32 with one rounding,
+ *   silu'(g) = s (1 + g (1 - s)), s = sigmoid(g);  dgu[:, F:] = bf16(dh * bf16(silu(g))), the value the forward used.
+ * Requirements: every pointer non-NULL, rows >= 1, F a positive multiple of 8, ldgu and lddgu >= 2F, ldh and lddh >= F
+ *   (OFK_ERR_ARG); every pointer 16-byte aligned and every stride a multiple of 8 (OFK_ERR_ALIGN).  Every argument is
+ *   checked before the first CUDA call. */
+int ofk_swiglu_fwd(const void* gu, long long ldgu, int rows, int F, void* h, long long ldh, void* stream);
+int ofk_swiglu_bwd(const void* dh, long long lddh, const void* gu, long long ldgu, int rows, int F, void* dgu,
+                   long long lddgu, void* stream);
 
 /* dst(f32) += src(f32) */
 int ofk_add_f32(float* dst, const float* src, long long n, void* stream);

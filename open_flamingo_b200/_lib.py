@@ -78,6 +78,11 @@ _SIGNATURES = {
                                     c_int, c_int, c_int, c_void_p, c_void_p, c_ll, c_ll, c_void_p, c_ll, c_ll,
                                     c_void_p]),
     "ofk_gelu_bf16": (c_int, [c_void_p, c_void_p, c_ll, c_void_p]),
+    "ofk_rmsnorm_fwd": (c_int, [c_void_p, c_ll, c_void_p, c_float, c_int, c_int, c_void_p, c_ll, c_void_p, c_void_p]),
+    "ofk_rmsnorm_bwd": (c_int, [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_void_p, c_int, c_int, c_void_p, c_ll,
+                                c_void_p, c_ll, c_void_p]),
+    "ofk_swiglu_fwd": (c_int, [c_void_p, c_ll, c_int, c_int, c_void_p, c_ll, c_void_p]),
+    "ofk_swiglu_bwd": (c_int, [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_void_p, c_ll, c_void_p]),
     "ofk_text_time": (c_int, [c_void_p, c_ll, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "ofk_cast_f32_bf16": (c_int, [c_void_p, c_void_p, c_ll, c_void_p]),
     "ofk_reduce_workspace_bytes": (c_ll, []),

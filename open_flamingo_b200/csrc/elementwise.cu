@@ -108,6 +108,65 @@ __global__ void gelu_bf16_kernel(const uint4* __restrict__ z, uint4* __restrict_
   }
 }
 
+// ---- SwiGLU of the LLaMA MLP (HF LlamaMLP: act_fn(gate_proj(x)) * up_proj(x)), on the output gu = [g | u] of one
+// GEMM against the concatenated gate|up weight.  silu is torch's x / (1 + exp(-x)) in fp32, rounded to bf16 as
+// autocast rounds act_fn's output; exp(-g) = inf for very negative g gives -0, never NaN.
+__device__ __forceinline__ float silu_bf16(float g) { return bf16_round(g / (1.0f + expf(-g))); }
+
+// h = bf16(bf16(silu(g)) * u): one 8-column group of one row per item.
+__global__ void swiglu_fwd_kernel(const __nv_bfloat16* __restrict__ gu, long long ldgu, int F,
+                                  __nv_bfloat16* __restrict__ h, long long ldh, long long n8) {
+  const int f8 = F / 8;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += stride) {
+    const long long r = i / f8;
+    const int c = (int)(i % f8) * 8;
+    const uint4 g = *reinterpret_cast<const uint4*>(gu + r * ldgu + c);
+    const uint4 u = *reinterpret_cast<const uint4*>(gu + r * ldgu + F + c);
+    const uint32_t gw[4] = {g.x, g.y, g.z, g.w}, uw[4] = {u.x, u.y, u.z, u.w};
+    uint32_t o[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      o[j] = pack_bf16x2(silu_bf16(bf16_lo(gw[j])) * bf16_lo(uw[j]), silu_bf16(bf16_hi(gw[j])) * bf16_hi(uw[j]));
+    *reinterpret_cast<uint4*>(h + r * ldh + c) = make_uint4(o[0], o[1], o[2], o[3]);
+  }
+}
+
+// dg = bf16(dh * u * silu'(g)), silu'(g) = s (1 + g (1 - s)) with s = sigmoid(g), in fp32 with one rounding;
+// du = bf16(dh * bf16(silu(g))), the silu value the forward multiplied by.
+__global__ void swiglu_bwd_kernel(const __nv_bfloat16* __restrict__ dh, long long lddh,
+                                  const __nv_bfloat16* __restrict__ gu, long long ldgu, int F,
+                                  __nv_bfloat16* __restrict__ dgu, long long lddgu, long long n8) {
+  const int f8 = F / 8;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += stride) {
+    const long long r = i / f8;
+    const int c = (int)(i % f8) * 8;
+    const uint4 d = *reinterpret_cast<const uint4*>(dh + r * lddh + c);
+    const uint4 g = *reinterpret_cast<const uint4*>(gu + r * ldgu + c);
+    const uint4 u = *reinterpret_cast<const uint4*>(gu + r * ldgu + F + c);
+    const uint32_t dw[4] = {d.x, d.y, d.z, d.w}, gw[4] = {g.x, g.y, g.z, g.w}, uw[4] = {u.x, u.y, u.z, u.w};
+    uint32_t og[4], ou[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      float dg2[2], du2[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float dv = e ? bf16_hi(dw[j]) : bf16_lo(dw[j]);
+        const float gv = e ? bf16_hi(gw[j]) : bf16_lo(gw[j]);
+        const float uv = e ? bf16_hi(uw[j]) : bf16_lo(uw[j]);
+        const float sg = 1.0f / (1.0f + expf(-gv));
+        dg2[e] = (dv * uv) * (sg * (1.0f + gv * (1.0f - sg)));
+        du2[e] = dv * silu_bf16(gv);
+      }
+      og[j] = pack_bf16x2(dg2[0], dg2[1]);
+      ou[j] = pack_bf16x2(du2[0], du2[1]);
+    }
+    *reinterpret_cast<uint4*>(dgu + r * lddgu + c) = make_uint4(og[0], og[1], og[2], og[3]);
+    *reinterpret_cast<uint4*>(dgu + r * lddgu + F + c) = make_uint4(ou[0], ou[1], ou[2], ou[3]);
+  }
+}
+
 // ---- gate backward: dbranch = dout * tanh(g) (bf16); dgate += (1 - tanh(g)^2) * <dout, branch>
 __global__ void __launch_bounds__(256) gate_bwd_kernel(const float* __restrict__ dout, const __nv_bfloat16* __restrict__ branch,
                                                        const float* __restrict__ gate, __nv_bfloat16* __restrict__ dbranch,
@@ -306,6 +365,46 @@ extern "C" int ofk_gelu_bf16(const void* z, void* h, long long n, void* stream) 
   if (n % 8 != 0) return ofk_set_error(OFK_ERR_ARG, "gelu: n must be a multiple of 8");
   if (misaligned(z, 16) || misaligned(h, 16)) return ofk_set_error(OFK_ERR_ALIGN, "gelu: pointers must be 16-byte aligned");
   gelu_bf16_kernel<<<grid_for(n / 8, 256), 256, 0, (cudaStream_t)stream>>>((const uint4*)z, (uint4*)h, n / 8);
+  OFK_CHECK_LAUNCH();
+  return 0;
+}
+
+// The checks both SwiGLU directions share: rows and F, then the strides of the [rows, 2F] and [rows, F] operands.
+static int swiglu_check(const char* what, int rows, int F, long long ld_wide, long long ld_narrow) {
+  if (rows < 1) return ofk_set_error(OFK_ERR_ARG, what);
+  if (F < 1 || F % 8 != 0) return ofk_set_error(OFK_ERR_ARG, what);
+  if (ld_wide < 2LL * F || ld_narrow < F) return ofk_set_error(OFK_ERR_ARG, what);
+  if (ld_wide % 8 != 0 || ld_narrow % 8 != 0) return ofk_set_error(OFK_ERR_ALIGN, what);
+  return 0;
+}
+
+extern "C" int ofk_swiglu_fwd(const void* gu, long long ldgu, int rows, int F, void* h, long long ldh, void* stream) {
+  if (!gu || !h) return ofk_set_error(OFK_ERR_ARG, "swiglu: null pointer");
+  if (int rc = swiglu_check("swiglu: rows >= 1, F a positive multiple of 8, ldgu >= 2F and ldh >= F, strides multiples "
+                            "of 8", rows, F, ldgu, ldh))
+    return rc;
+  if (misaligned(gu, 16) || misaligned(h, 16)) return ofk_set_error(OFK_ERR_ALIGN, "swiglu: gu and h must be 16-byte aligned");
+  const long long n8 = (long long)rows * (F / 8);
+  swiglu_fwd_kernel<<<grid_for(n8, 256), 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)gu, ldgu, F,
+                                                                          (__nv_bfloat16*)h, ldh, n8);
+  OFK_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int ofk_swiglu_bwd(const void* dh, long long lddh, const void* gu, long long ldgu, int rows, int F, void* dgu,
+                              long long lddgu, void* stream) {
+  if (!dh || !gu || !dgu) return ofk_set_error(OFK_ERR_ARG, "swiglu bwd: null pointer");
+  if (int rc = swiglu_check("swiglu bwd: rows >= 1, F a positive multiple of 8, ldgu and lddgu >= 2F, lddh >= F, "
+                            "strides multiples of 8", rows, F, ldgu, lddh))
+    return rc;
+  if (lddgu < 2LL * F) return ofk_set_error(OFK_ERR_ARG, "swiglu bwd: lddgu must be >= 2F");
+  if (lddgu % 8 != 0) return ofk_set_error(OFK_ERR_ALIGN, "swiglu bwd: lddgu must be a multiple of 8");
+  if (misaligned(dh, 16) || misaligned(gu, 16) || misaligned(dgu, 16))
+    return ofk_set_error(OFK_ERR_ALIGN, "swiglu bwd: dh, gu and dgu must be 16-byte aligned");
+  const long long n8 = (long long)rows * (F / 8);
+  swiglu_bwd_kernel<<<grid_for(n8, 256), 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)dh, lddh,
+                                                                          (const __nv_bfloat16*)gu, ldgu, F,
+                                                                          (__nv_bfloat16*)dgu, lddgu, n8);
   OFK_CHECK_LAUNCH();
   return 0;
 }

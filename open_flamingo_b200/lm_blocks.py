@@ -1,5 +1,6 @@
-"""Frozen-LM decoder blocks on the sm_90a kernels (SURVEY.md section 8f, rank 1): HF `MptBlock` (OF-3B, OF-9B) and
-HF `GPTNeoXLayer` (OF-4B; see the GPT-NeoX section below).
+"""Frozen-LM decoder blocks on the sm_90a kernels (SURVEY.md section 8f, rank 1): HF `MptBlock` (OF-3B, OF-9B),
+HF `GPTNeoXLayer` (OF-4B; see the GPT-NeoX section below) and HF `LlamaDecoderLayer` (OF-9B v1; see the LLaMA
+section).
 
 The reference runs the frozen LM's decoder block as ordinary PyTorch (`self.decoder_layer(lang_x, ...)`,
 flamingo_lm.py:63-65).  For the LM family named by BASELINE.json (MPT: HF `MptBlock` = LN -> Wqkv -> causal
@@ -625,11 +626,293 @@ class FastNeoXBlock:
         return out if out.dtype == hidden_states.dtype else out.to(hidden_states.dtype)
 
 
+# ---- LLaMA (HF LlamaDecoderLayer: the LM of the OpenFlamingo-9B v1 checkpoint, LLaMA-7B) -------------------------------
+#
+#   a = rmsnorm1(x);  q, k, v = a Wq^T, a Wk^T, a Wv^T;  q, k = rotary(q, k; cos, sin)     (rotate_half, full head)
+#   x1 = x + softmax(q k^T / sqrt(hd) + mask) v Wo^T
+#   out = x1 + (silu(g) * u) Wd^T,   g, u = rmsnorm2(x1) Wg^T, rmsnorm2(x1) Wu^T             no biases anywhere
+#
+# Under autocast HF rounds to bf16 at: the RMSNorm outputs (as Linear operands), every Linear output, q and k after the
+# rotation (as sdpa operands), silu(g) and silu(g) * u.  The kernels round at the same points: ofk_rmsnorm_fwd, the
+# STORE_BF16 / GATE_RESID_F32 GEMM epilogues, ofk_rope_pack and ofk_swiglu_fwd.
+#
+# Q, K and V come from one GEMM against one bf16 copy of [Wq; Wk; Wv] whose rows are re-ordered per head as
+# (q | k | v) -- the GPT-NeoX query_key_value layout -- so ofk_rope_pack splits and rotates its output and
+# ofk_rope_unpack_bwd writes the gradient the dgrad GEMM with the same copy takes.  Likewise g and u come from one GEMM
+# against a bf16 [Wg; Wu].  These packed copies are the only bf16 copies of those five weights.
+
+_wpack_cache = {}
+
+
+def _packed_w16(layout, params, fill):
+    """The bf16 weight `fill(params)` builds from several fp32 parameters, kept until one of them changes.  `layout`
+    names everything besides the parameters that `fill` reads (it is part of the cache key, so the same parameters
+    packed another way get their own copy).  Refreshed by w16's rule -- weakly referenced parameters at the same
+    version counters and addresses -- so `load_state_dict` or an in-place edit is seen."""
+    key = (layout,) + tuple(id(p) for p in params)
+    state = tuple((p._version, p.data_ptr()) for p in params)
+    ent = _wpack_cache.get(key)
+    if ent is not None and all(r() is p for r, p in zip(ent[0], params)) and ent[1] == state:
+        return ent[2]
+    t = fill(params)
+    refs = tuple(weakref.ref(p, lambda _r, k=key: _wpack_cache.pop(k, None)) for p in params)
+    _wpack_cache[key] = (refs, state, t)
+    return t
+
+
+def _qkv16(wq, wk, wv, heads):
+    """bf16 [3D, D] copy of the q/k/v projections with rows in the per-head (q | k | v) order: packed row
+    (h * 3 + p) * hd + j is row j of head h of part p (Wq, Wk, Wv)."""
+    def fill(ps):
+        D, K = ps[0].shape
+        t = torch.empty((heads, 3, D // heads, K), device=ps[0].device, dtype=bf16)
+        for i, p in enumerate(ps):
+            t[:, i].copy_(p.detach().view(heads, D // heads, K))
+        return t.view(3 * D, K)
+    return _packed_w16(("qkv", heads), (wq, wk, wv), fill)
+
+
+def _gu16(wg, wu):
+    """bf16 [2F, D] copy of cat([Wg, Wu]): the gate|up GEMM writes gu = [g | u]."""
+    def fill(ps):
+        F, K = ps[0].shape
+        t = torch.empty((2 * F, K), device=ps[0].device, dtype=bf16)
+        t[:F].copy_(ps[0].detach())
+        t[F:].copy_(ps[1].detach())
+        return t
+    return _packed_w16("gate|up", (wg, wu), fill)
+
+
+def _llama_tail(x2d, o, eps2, wo, n2_w, wg, wu, wd, want_rstd):
+    """The block after its attention core.  x2d: [R, D] f32 block input; o: [R, D] bf16 attention output.  Returns
+    (out, x1, rstd2, gu): x1 = x + bf16(o Wo^T), the second RMSNorm's rstd (None unless want_rstd) and gu = [g | u]."""
+    x1 = ops.gemm(o, w16(wo), epi=L.EPI_GATE_RESID_F32, aux=x2d)                   # + residual
+    a2, rstd2 = ops.rmsnorm_fwd(x1, n2_w, eps2, want_rstd=want_rstd)
+    gu = ops.gemm(a2, _gu16(wg, wu))                                                # [R, 2F]
+    del a2
+    h = ops.swiglu_fwd(gu)
+    out = ops.gemm(h, w16(wd), epi=L.EPI_GATE_RESID_F32, aux=x1)                    # + residual
+    return out, x1, rstd2, gu
+
+
+class FrozenLlamaBlockFn(torch.autograd.Function):
+    """A frozen LlamaDecoderLayer: forward, and the backward to its input only (the parameters take no gradient).
+    x: [B, T, D] f32; mask: [B, T, T] bytes (nonzero = masked) or None for causal only; cos, sin: f32 [1 or B, T, rot]."""
+
+    @staticmethod
+    def forward(ctx, x, mask, pure_flag, cos, sin, heads, eps1, eps2, n1_w, wq, wk, wv, wo, n2_w, wg, wu, wd):
+        B, T, D = x.shape
+        R = B * T
+        hd = D // heads
+        x2d = _rows(x)
+        a, rstd1 = ops.rmsnorm_fwd(x2d, n1_w, eps1)
+        qkv = ops.gemm(a, _qkv16(wq, wk, wv, heads))                                # [R, 3D], heads as (q | k | v)
+        del a
+        q, k, v = ops.rope_pack(qkv.view(B, T, 3 * D), heads, hd, cos, sin)
+        del qkv
+        scale = float(hd ** -0.5)
+        o, lse = ops.attn_dense_fwd(q, k, v, heads, hd, scale, causal=mask is None, mask=mask,
+                                    pure_causal_flag=pure_flag)
+        out, x1, rstd2, gu = _llama_tail(x2d, o.view(R, D), eps2, wo, n2_w, wg, wu, wd, want_rstd=True)
+        ctx.save_for_backward(x2d, rstd1, q, k, v, o, lse, x1, rstd2, gu, cos, sin, n1_w, wq, wk, wv, wo, n2_w, wg, wu,
+                              wd, mask if mask is not None else x2d.new_empty(0),
+                              pure_flag if pure_flag is not None else x2d.new_empty(0))
+        ctx.meta = (B, T, D, heads, hd, scale, mask is not None, pure_flag is not None)
+        return out.view(B, T, D)
+
+    @staticmethod
+    def backward(ctx, dout):
+        (x2d, rstd1, q, k, v, o, lse, x1, rstd2, gu, cos, sin, n1_w, wq, wk, wv, wo, n2_w, wg, wu, wd, mask,
+         pure_flag) = ctx.saved_tensors
+        B, T, D, heads, hd, scale, has_mask, has_flag = ctx.meta
+        mask = mask if has_mask else None
+        pure_flag = pure_flag if has_flag else None
+        R = B * T
+        d2 = _rows(dout)
+        if d2.dtype != f32:
+            d2 = d2.float()
+        dbr = ops.gate_bwd(d2, None, None, None)                                     # bf16 cast
+        dh = ops.gemm(dbr, w16(wd), b_mn=True)                                       # [R, F]
+        del dbr
+        dgu = ops.swiglu_bwd(dh, gu)                                                 # [R, 2F]
+        del dh
+        da2 = ops.gemm(dgu, _gu16(wg, wu), b_mn=True)
+        del dgu
+        dx1 = ops.rmsnorm_bwd(da2, x1, n2_w, rstd2, dx_add=d2)
+        del da2
+        dy = ops.gate_bwd(dx1, None, None, None)
+        d_o = ops.gemm(dy, w16(wo), b_mn=True)                                       # [R, D]
+        del dy
+        dq, dk, dv = ops.attn_dense_bwd(q, k, v, o, d_o.view(B, T, D), lse, heads, hd, scale,
+                                        causal=mask is None, mask=mask, pure_causal_flag=pure_flag)
+        del d_o
+        dqkv = ops.rope_unpack_bwd(dq, dk, dv, heads, hd, cos, sin)                  # [B, T, 3D]
+        del dq, dk, dv
+        da = ops.gemm(dqkv.view(R, 3 * D), _qkv16(wq, wk, wv, heads), b_mn=True)
+        dx = ops.rmsnorm_bwd(da, x2d, n1_w, rstd1, dx_add=dx1)
+        return (dx.view(B, T, D),) + (None,) * 16
+
+
+def cached_llama_block_forward(x, layer, mask, pure_flag, cos, sin, heads, eps1, eps2, n1_w, wq, wk, wv, wo, n2_w, wg,
+                               wu, wd):
+    """Inference forward of one LLaMA block that appends its nq new tokens to `layer` (a kv_cache.KVCacheLayer) and
+    attends over everything cached.  ops.rope_pack writes the rotated K and the V straight into cache rows
+    [past, past + nq); one token attends through the decode kernel, a chunk through the dense kernel over the cached
+    views.  mask: as for cached_block_forward.  x: [B, nq, D] f32; returns the same."""
+    B, nq, D = x.shape
+    hd = D // heads
+    x2d = _rows(x)
+    a, _ = ops.rmsnorm_fwd(x2d, n1_w, eps1, want_rstd=False)
+    qkv = ops.gemm(a, _qkv16(wq, wk, wv, heads)).view(B, nq, 3 * D)
+    del a
+    if not layer.is_initialized:
+        layer.init_storage(B, heads, hd, bf16, x.device)
+    past = layer.length
+    rows = layer.reserve(nq)[:, past:past + nq]
+    q, _, _ = ops.rope_pack(qkv, heads, hd, cos, sin, k=rows[..., :D], v=rows[..., D:])
+    del qkv
+    layer.length = past + nq
+    k, v = layer.kv_views()
+    scale = float(hd ** -0.5)
+    if nq == 1:
+        o = ops.attn_decode(q.view(B, D), k, v, heads, hd, scale, key_mask=mask)
+    else:
+        o, _ = ops.attn_dense_fwd(q, k, v, heads, hd, scale, causal=mask is None, mask=mask, pure_causal_flag=pure_flag,
+                                  want_lse=False)
+    return _llama_tail(x2d, o.view(B * nq, D), eps2, wo, n2_w, wg, wu, wd, want_rstd=False)[0].view(B, nq, D)
+
+
+class FastLlamaBlock:
+    """Callable with HF LlamaDecoderLayer.forward's signature; returns None when the fast path does not apply, and the
+    block's output tensor otherwise.
+
+    Graph-replayed decoding does not cover LLaMA: decode_graph.eligible declines an LM that is neither GPT-NeoX nor
+    has MPT's `transformer` / `norm_f`, so `generate(..., cache_implementation="static")` runs the eager cached path
+    on the fixed-capacity KVCache, step by step.  Those steps are the ones a growing KVCache takes (the same kernels
+    on the same rows; the decode kernel's split does not depend on the capacity), so they give the same bits."""
+
+    def __init__(self, block):
+        self.block = block
+
+    def records_outputs(self, output_attentions=None, output_hidden_states=None):
+        """Whether the caller asked HF to record this layer's hidden states or attention weights, which LlamaModel
+        does with hooks on the modules the fast path does not call (see FastNeoXBlock.records_outputs)."""
+        cfg = self.block.self_attn.config
+        if output_attentions is None:
+            output_attentions = getattr(cfg, "output_attentions", False)
+        if output_hidden_states is None:
+            output_hidden_states = getattr(cfg, "output_hidden_states", False)
+        return bool(output_attentions or output_hidden_states)
+
+    def supported(self, hidden_states, position_embeddings, record_outputs):
+        """The block and call are ones the kernels evaluate, whatever the cache."""
+        if position_embeddings is None or not self.block_supported(hidden_states, record_outputs):
+            return False
+        cos, sin = position_embeddings
+        if cos.dtype != f32 or sin.dtype != f32 or cos.dim() != 3 or cos.shape != sin.shape or \
+                cos.stride() != sin.stride() or cos.stride(2) != 1 or cos.shape[2] % 2 or \
+                not 0 < cos.shape[2] <= self.block.self_attn.head_dim:
+            return False
+        return True
+
+    def block_supported(self, hidden_states, record_outputs):
+        """The part of `supported` that does not read the rotary tables."""
+        b = self.block
+        a = b.self_attn
+        cfg = a.config
+        if not ENABLED or not hidden_states.is_cuda or record_outputs:
+            return False
+        hd = a.head_dim
+        if hd not in (64, 128) or abs(a.scaling - hd ** -0.5) > 1e-9:
+            return False
+        if cfg.num_key_value_heads != cfg.num_attention_heads or cfg.num_attention_heads * hd != cfg.hidden_size:
+            return False   # grouped-query attention needs a K/V head map the cores do not have
+        if getattr(cfg, "hidden_act", None) != "silu" or b.mlp.intermediate_size % 16:
+            return False   # the GEMMs take N % 16 == 0, the down-projection's dgrad has N = intermediate_size
+        if b.training and a.attention_dropout > 0:
+            return False
+        lins = (a.q_proj, a.k_proj, a.v_proj, a.o_proj, b.mlp.gate_proj, b.mlp.up_proj, b.mlp.down_proj)
+        if any(m.bias is not None for m in lins) or any(p.dtype != f32 for p in b.parameters()):
+            return False
+        if any(p.requires_grad for p in b.parameters()):
+            return False   # this path has no wgrad: frozen blocks only
+        return True
+
+    def weights(self):
+        b = self.block
+        a = b.self_attn
+        m = b.mlp
+        return (b.input_layernorm.weight, a.q_proj.weight, a.k_proj.weight, a.v_proj.weight, a.o_proj.weight,
+                b.post_attention_layernorm.weight, m.gate_proj.weight, m.up_proj.weight, m.down_proj.weight)
+
+    def step_args(self):
+        """The head count and RMSNorm eps of the block, then its weights: the arguments after cos and sin of
+        cached_llama_block_forward."""
+        b = self.block
+        return (b.self_attn.config.num_attention_heads, b.input_layernorm.variance_epsilon,
+                b.post_attention_layernorm.variance_epsilon) + self.weights()
+
+    def applicable(self, hidden_states, position_embeddings, past_key_values, use_cache, record_outputs):
+        """The uncached path (FrozenLlamaBlockFn, forward and backward)."""
+        if past_key_values is not None or use_cache:
+            return False
+        return self.supported(hidden_states, position_embeddings, record_outputs)
+
+    def cache_layer(self, hidden_states, position_embeddings, past_key_values, record_outputs):
+        """The KVCacheLayer the cached path appends to, or None (see FastMptBlock.cache_layer)."""
+        if not isinstance(past_key_values, KVCache) or torch.is_grad_enabled():
+            return None
+        if not self.supported(hidden_states, position_embeddings, record_outputs):
+            return None
+        a = self.block.self_attn
+        if a.layer_idx is None or not 0 <= a.layer_idx < len(past_key_values.layers):
+            return None
+        layer = past_key_values.layers[a.layer_idx]
+        if layer.is_initialized and (layer.buf.dtype != bf16 or layer.buf.device != hidden_states.device or
+                                     layer.buf.shape[0] != hidden_states.shape[0] or
+                                     layer.heads != a.config.num_attention_heads or layer.head_dim != a.head_dim):
+            return None
+        return layer
+
+    def __call__(self, hidden_states, attention_mask=None, position_ids=None, past_key_values=None, use_cache=False,
+                 position_embeddings=None, output_attentions=None, output_hidden_states=None, pure_causal_flag=None,
+                 **kwargs):
+        record = self.records_outputs(output_attentions, output_hidden_states)
+        layer = None
+        if past_key_values is not None or use_cache:
+            layer = self.cache_layer(hidden_states, position_embeddings, past_key_values, record)
+            if layer is None:
+                return None
+        elif not self.applicable(hidden_states, position_embeddings, past_key_values, use_cache, record):
+            return None
+        B, T, _ = hidden_states.shape
+        cos, sin = position_embeddings
+        if cos.shape[0] not in (1, B) or cos.shape[1] != T:
+            return None
+        nk = T if layer is None else layer.length + T
+        mask = None
+        if attention_mask is not None:   # HF's sdpa mask, True = attend; a float (eager) mask is declined here
+            mask = _kernel_mask(attention_mask, B, T, nk, layer is not None and T == 1, true_attends=True)
+            if mask is None:
+                return None
+        x = hidden_states if hidden_states.dtype == f32 else hidden_states.float()
+        flag = pure_causal_flag if mask is not None else None
+        rest = (cos, sin) + self.step_args()
+        if layer is not None:
+            out = cached_llama_block_forward(x, layer, mask, flag, *rest)
+        else:
+            out = FrozenLlamaBlockFn.apply(x, mask, flag, *rest)
+        return out if out.dtype == hidden_states.dtype else out.to(hidden_states.dtype)
+
+
 def accelerate(decoder_layer):
-    """Return a fast evaluator for a recognised frozen decoder block (HF MptBlock or GPTNeoXLayer), else None."""
+    """Return a fast evaluator for a recognised frozen decoder block (HF MptBlock, GPTNeoXLayer or LlamaDecoderLayer),
+    else None."""
     name = type(decoder_layer).__name__
     if name == "MptBlock" and hasattr(decoder_layer, "attn") and hasattr(decoder_layer, "ffn"):
         return FastMptBlock(decoder_layer)
     if name == "GPTNeoXLayer" and hasattr(decoder_layer, "attention") and hasattr(decoder_layer, "mlp"):
         return FastNeoXBlock(decoder_layer)
+    if name == "LlamaDecoderLayer" and hasattr(decoder_layer, "self_attn") and hasattr(decoder_layer, "mlp"):
+        return FastLlamaBlock(decoder_layer)
     return None

@@ -755,3 +755,81 @@ def gelu_bf16(z, out=None):
     _vector(out, "out", bf16, z.numel())
     L.check(L.lib().ofk_gelu_bf16(z.data_ptr(), out.data_ptr(), z.numel(), L.stream_ptr()))
     return out
+
+
+def rmsnorm_fwd(x, gamma, eps, *, out=None, want_rstd=True):
+    """RMSNorm (ofk_rmsnorm_fwd): x [rows, D] f32 with unit inner stride -> (y, rstd): y = bf16(gamma * (x * rstd))
+    [rows, D] (`out`, allocated when None), rstd [rows] f32 (None unless want_rstd)."""
+    L.require_cuda(x, gamma, out)
+    _rowmajor_2d(x, "x")
+    if x.dtype != f32:
+        raise ValueError("rmsnorm input must be float32 (the residual stream is fp32)")
+    rows, D = x.shape
+    _vector(gamma, "gamma", f32, D)
+    if out is None:
+        out = torch.empty((rows, D), device=x.device, dtype=bf16)
+    _rows2d(out, "out", (bf16,), rows, D)
+    rstd = torch.empty(rows, device=x.device, dtype=f32) if want_rstd else None
+    if rows:
+        L.check(L.lib().ofk_rmsnorm_fwd(x.data_ptr(), x.stride(0), gamma.data_ptr(), float(eps), rows, D,
+                                        out.data_ptr(), out.stride(0), L.ptr(rstd), L.stream_ptr()))
+    return out, rstd
+
+
+def rmsnorm_bwd(dy, x, gamma, rstd, *, dx=None, dx_add=None):
+    """Input gradient of rmsnorm_fwd (ofk_rmsnorm_bwd): dy [rows, D] bf16 -> dx [rows, D] f32 (`dx`, allocated when
+    None) = rstd * (gamma * dy - xhat * mean(gamma * dy * xhat)) + dx_add; dx_add may be dx itself."""
+    L.require_cuda(dy, x, gamma, rstd, dx, dx_add)
+    _rowmajor_2d(x, "x")
+    if x.dtype != f32:
+        raise ValueError("rmsnorm input must be float32 (the residual stream is fp32)")
+    rows, D = x.shape
+    _rows2d(dy, "dy", (bf16,), rows, D)
+    _vector(gamma, "gamma", f32, D)
+    _vector(rstd, "rstd", f32, rows)
+    for t, name in ((dx, "dx"), (dx_add, "dx_add")):
+        if t is not None:
+            _rows2d(t, name, (f32,), rows, D)
+    if dx is None:
+        dx = torch.empty((rows, D), device=x.device, dtype=f32)
+    if rows:
+        L.check(L.lib().ofk_rmsnorm_bwd(dy.data_ptr(), dy.stride(0), x.data_ptr(), x.stride(0), gamma.data_ptr(),
+                                        rstd.data_ptr(), rows, D, dx.data_ptr(), dx.stride(0), L.ptr(dx_add),
+                                        0 if dx_add is None else dx_add.stride(0), L.stream_ptr()))
+    return dx
+
+
+def _swiglu_gu(gu):
+    _rowmajor_2d(gu, "gu")
+    if gu.dtype != bf16 or gu.shape[1] % 2:
+        raise ValueError(f"gu must be bf16 [rows, 2F], got {tuple(gu.shape)} {gu.dtype}")
+    return gu.shape[0], gu.shape[1] // 2
+
+
+def swiglu_fwd(gu, out=None):
+    """SwiGLU (ofk_swiglu_fwd): gu = [g | u] bf16 [rows, 2F] -> h = bf16(bf16(silu(g)) * u) [rows, F] (`out`,
+    allocated when None)."""
+    L.require_cuda(gu, out)
+    rows, F = _swiglu_gu(gu)
+    if out is None:
+        out = torch.empty((rows, F), device=gu.device, dtype=bf16)
+    _rows2d(out, "out", (bf16,), rows, F)
+    if rows:
+        L.check(L.lib().ofk_swiglu_fwd(gu.data_ptr(), gu.stride(0), rows, F, out.data_ptr(), out.stride(0),
+                                       L.stream_ptr()))
+    return out
+
+
+def swiglu_bwd(dh, gu, out=None):
+    """Gradient of swiglu_fwd (ofk_swiglu_bwd): dh bf16 [rows, F] -> dgu bf16 [rows, 2F] (`out`, allocated when
+    None): [bf16(dh * u * silu'(g)) | bf16(dh * bf16(silu(g)))]."""
+    L.require_cuda(dh, gu, out)
+    rows, F = _swiglu_gu(gu)
+    _rows2d(dh, "dh", (bf16,), rows, F)
+    if out is None:
+        out = torch.empty((rows, 2 * F), device=gu.device, dtype=bf16)
+    _rows2d(out, "out", (bf16,), rows, 2 * F)
+    if rows:
+        L.check(L.lib().ofk_swiglu_bwd(dh.data_ptr(), dh.stride(0), gu.data_ptr(), gu.stride(0), rows, F,
+                                       out.data_ptr(), out.stride(0), L.stream_ptr()))
+    return out

@@ -32,8 +32,9 @@ class FlamingoLayer(nn.Module):
         self.vis_x = None
         self.media_locations = None
         self.use_cached_media = None
-        # recognised frozen decoder blocks (HF MptBlock, GPTNeoXLayer) are evaluated on the sm_90a kernels; everything
-        # else -- and every case the fast path declines -- runs the block's own PyTorch forward as in the reference
+        # recognised frozen decoder blocks (HF MptBlock, GPTNeoXLayer, LlamaDecoderLayer) are evaluated on the sm_90a
+        # kernels; everything else -- and every case the fast path declines -- runs the block's own PyTorch forward as
+        # in the reference
         self._fast_block = lm_blocks.accelerate(decoder_layer)
         self._pure_causal_flag = None
         # kept for API compatibility (train.py:368-381); the fused blocks already store only what backward needs
@@ -167,7 +168,7 @@ class FlamingoLMMixin(nn.Module):
     def make_kv_cache(self, capacity=None):
         """A kv_cache.KVCache for decoding this LM on the kernels, or None where HF's own cache is kept: it is made only
         on CUDA, under `torch.autocast("cuda", dtype=torch.bfloat16)` (the caller asked for bf16 numerics; the cache
-        stores bf16), with lm_blocks.ENABLED, and when every decoder block is a recognised MPT or GPT-NeoX block.  In
+        stores bf16), with lm_blocks.ENABLED, and when every decoder block is a recognised MPT, GPT-NeoX or LLaMA block.  In
         fp32 every path stays HF's.
 
         capacity: None for a cache that grows; an int for a fixed-capacity cache of at least that many rows, with which

@@ -79,17 +79,37 @@ def build_neox(neox_kw, dtype=torch.float32, device="cpu", seed=0):
     return lm.to(dtype).eval()
 
 
+# LLaMA-7B, the LM of the OpenFlamingo-9B v1 checkpoint: D 4096, 32 heads of 128, 32 layers, FFN 11008.
+LLAMA_7B = dict(hidden_size=4096, num_attention_heads=32, num_key_value_heads=32, num_hidden_layers=32,
+                intermediate_size=11008, vocab_size=32000, max_position_embeddings=2048, rms_norm_eps=1e-6)
+
+
+def build_llama(llama_kw, dtype=torch.float32, device="cpu", seed=0):
+    """Random-init HF LlamaForCausalLM from a LlamaConfig (offline), attention through sdpa, whose boolean mask is what
+    the kernels take."""
+    from transformers import LlamaConfig, LlamaForCausalLM
+    torch.manual_seed(seed)
+    cfg = LlamaConfig(**llama_kw, attn_implementation="sdpa")
+    with torch.device(device):
+        lm = LlamaForCausalLM(cfg)
+    return lm.to(dtype).eval()
+
+
 def build_flamingo(vit_cfg, mpt_kw, cross_attn_every_n_layers=1, device="cuda", freeze_lm_embeddings=True, seed=0,
-                   lm_dtype=torch.float32, gate_init=None, neox_kw=None):
+                   lm_dtype=torch.float32, gate_init=None, neox_kw=None, llama_kw=None):
     """Random-init Flamingo through the public factory.  gate_init: None keeps the reference's zero gates
     (helpers.py:255,258); a float f draws gates ~ U(-f, f) so the gated path is actually exercised.  neox_kw: build
-    the LM with build_neox(neox_kw) instead of an MPT from mpt_kw (pass mpt_kw=None)."""
+    the LM with build_neox(neox_kw) instead of an MPT from mpt_kw (pass mpt_kw=None); llama_kw likewise with
+    build_llama."""
     torch.manual_seed(seed)
     with torch.device(device):
         vit = VisionTransformer(**vit_cfg)
     if neox_kw is not None:
         lm = build_neox(neox_kw, dtype=lm_dtype, device=device, seed=seed + 1)
         base_vocab = neox_kw["vocab_size"]
+    elif llama_kw is not None:
+        lm = build_llama(llama_kw, dtype=lm_dtype, device=device, seed=seed + 1)
+        base_vocab = llama_kw["vocab_size"]
     else:
         lm = build_mpt(mpt_kw, dtype=lm_dtype, device=device, seed=seed + 1)
         base_vocab = mpt_kw["vocab_size"]
