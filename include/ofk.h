@@ -358,6 +358,34 @@ int ofk_swiglu_fwd(const void* gu, long long ldgu, int rows, int F, void* h, lon
 int ofk_swiglu_bwd(const void* dh, long long lddh, const void* gu, long long ldgu, int rows, int F, void* dgu,
                    long long lddgu, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * CLIP image preprocessing: open_clip's eval transform (image_transform(is_train=False), the image_processor that
+ * create_model_and_transforms returns, factory.py:42) on decoded uint8 pixels:
+ *   Resize(S, BICUBIC) + CenterCrop(S) + ToTensor + Normalize(mean, std)
+ * bit for bit what torchvision + Pillow compute from the same PIL image in mode RGB (c = 3) or L (c = 1; resampled as
+ * one channel and replicated to R = G = B after the crop, as open_clip's _convert_to_rgb runs after the crop).
+ *   Resize: the shorter side becomes S, the longer int(S * long / short); Pillow's two-pass fixed-point bicubic
+ *     (a = -0.5, int32 taps at 22 fractional bits, uint8 intermediate), horizontal pass first unless the image is more
+ *     than 100 times taller than wide and its height shrinks (Image.resize's order).
+ *   CenterCrop: top = round((H - S) / 2), left = round((W - S) / 2), half to even.  Only the crop window is computed.
+ *   out = ((float)u8 / 255 - mean[c]) / std[c] in IEEE fp32.
+ * shape: host int64 [n][4] = (h, w, c, row stride in bytes) per image; pixels are HWC uint8 rows.  Requirements: n in
+ *   [1, 65535], S in [1, 4096], h, w >= 1, S * max(h, w) < 2^31, c in {1, 3}, row stride >= w * c (OFK_ERR_ARG).
+ * ofk_image_plan_size: host only; writes the plan's size and the device workspace size (the plan's device copy plus
+ *   the uint8 intermediates).
+ * ofk_image_plan: host only; src: n device pointers (host array) to each image's pixel (0, 0); mean, std: 3 host floats
+ *   each, finite, std nonzero; plan: caller-owned host buffer of exactly plan_bytes, 16-byte aligned (OFK_ERR_ALIGN).
+ * ofk_clip_preprocess: checks the plan (every table and intermediate inside its bounds), copies it into `workspace`
+ *   (device, >= the workspace size, 16-byte aligned) on `stream` and makes two launches for the whole batch, writing
+ *   out[i] (f32 [3, S, S] at out + i * out_image_stride, stride >= 3 S^2, out 4-byte aligned).  A pageable plan may be
+ *   reused when the call returns; a pinned one once the stream has passed the copy.  Every argument is checked before
+ *   the first CUDA call. */
+int ofk_image_plan_size(int n, const long long* shape, int S, long long* plan_bytes, long long* workspace_bytes);
+int ofk_image_plan(int n, const void* const* src, const long long* shape, int S, const float* mean, const float* std_,
+                   void* plan, long long plan_bytes);
+int ofk_clip_preprocess(const void* plan, long long plan_bytes, void* workspace, long long workspace_bytes, float* out,
+                        long long out_image_stride, void* stream);
+
 /* dst(f32) += src(f32) */
 int ofk_add_f32(float* dst, const float* src, long long n, void* stream);
 

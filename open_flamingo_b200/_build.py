@@ -18,6 +18,9 @@ NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
+    # host double arithmetic rounds every operation (the image plan's bicubic taps must equal Pillow's, which rounds
+    # each product and sum; a contracted multiply-add on an FMA host would change them)
+    "-Xcompiler", "-ffp-contract=off",
     "--expt-relaxed-constexpr",
 ]
 

@@ -97,6 +97,9 @@ _SIGNATURES = {
     "ofk_adamw": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_float, c_float, c_float,
                           c_float, c_float, c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
     "ofk_sumsq": (c_int, [c_void_p, c_ll, c_void_p, c_void_p, c_void_p]),
+    "ofk_image_plan_size": (c_int, [c_int, c_void_p, c_int, c_void_p, c_void_p]),
+    "ofk_image_plan": (c_int, [c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_ll]),
+    "ofk_clip_preprocess": (c_int, [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p]),
 }
 
 _lib = None

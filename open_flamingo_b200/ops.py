@@ -833,3 +833,49 @@ def swiglu_bwd(dh, gu, out=None):
         L.check(L.lib().ofk_swiglu_bwd(dh.data_ptr(), dh.stride(0), gu.data_ptr(), gu.stride(0), rows, F,
                                        out.data_ptr(), out.stride(0), L.stream_ptr()))
     return out
+
+
+def clip_preprocess(images, size, mean, std, *, out=None):
+    """open_clip's eval transform (Resize(size, BICUBIC) + CenterCrop(size) + ToTensor + Normalize(mean, std)) of
+    decoded images on the GPU, bit for bit torchvision + Pillow (ofk_image_plan + ofk_clip_preprocess: two launches for
+    the whole batch).  images: a non-empty list of uint8 CUDA tensors [h, w, c], c = 1 (L) or 3 (RGB), channels and
+    pixels contiguous, rows at any stride >= w * c.  Returns out: f32 [N, 3, size, size] (`out`, allocated when None;
+    each image contiguous, images at any stride >= 3 size^2, so it may be a window of a larger vision_x buffer)."""
+    import ctypes
+    if not isinstance(images, (list, tuple)) or not images:
+        raise ValueError("clip_preprocess needs a non-empty list of images")
+    L.require_cuda(*images, out)
+    S = int(size)
+    if not 1 <= S <= 4096:
+        raise ValueError(f"size must be in [1, 4096], got {size}")
+    if len(mean) != 3 or len(std) != 3:
+        raise ValueError("mean and std must have 3 entries")
+    shape = []
+    for i, t in enumerate(images):
+        if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] not in (1, 3) or t.shape[0] < 1 or t.shape[1] < 1:
+            raise ValueError(f"image {i} must be a uint8 [h, w, 1 or 3] tensor, got {tuple(t.shape)} {t.dtype}")
+        h, w, c = t.shape
+        if t.stride(2) != 1 or t.stride(1) != c or t.stride(0) < w * c:
+            raise ValueError(f"image {i} must have contiguous channels and pixels (strides (>= {w * c}, {c}, 1)), got "
+                             f"{t.stride()}")
+        shape.append((h, w, c, t.stride(0)))
+    n = len(images)
+    if out is None:
+        out = torch.empty((n, 3, S, S), device=images[0].device, dtype=f32)
+    if (out.dtype != f32 or out.dim() != 4 or tuple(out.shape) != (n, 3, S, S) or out.stride(3) != 1
+            or out.stride(2) != S or out.stride(1) != S * S or (n > 1 and out.stride(0) < 3 * S * S)):
+        raise ValueError(f"out must be f32 [{n}, 3, {S}, {S}] with each image contiguous, got {tuple(out.shape)} "
+                         f"{out.dtype} stride {out.stride()}")
+    shape_t = torch.tensor(shape, dtype=torch.int64)
+    src_t = torch.tensor([t.data_ptr() for t in images], dtype=torch.int64)
+    plan_bytes, ws_bytes = ctypes.c_longlong(), ctypes.c_longlong()
+    lib = L.lib()
+    L.check(lib.ofk_image_plan_size(n, shape_t.data_ptr(), S, ctypes.byref(plan_bytes), ctypes.byref(ws_bytes)))
+    plan = torch.empty(plan_bytes.value, dtype=torch.uint8)
+    floats3 = ctypes.c_float * 3
+    L.check(lib.ofk_image_plan(n, src_t.data_ptr(), shape_t.data_ptr(), S, floats3(*mean), floats3(*std),
+                               plan.data_ptr(), plan_bytes.value))
+    ws = torch.empty(ws_bytes.value, device=out.device, dtype=torch.uint8)
+    L.check(lib.ofk_clip_preprocess(plan.data_ptr(), plan_bytes.value, ws.data_ptr(), ws_bytes.value, out.data_ptr(),
+                                    out.stride(0) if n > 1 else 3 * S * S, L.stream_ptr()))
+    return out
