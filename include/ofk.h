@@ -80,7 +80,8 @@ int ofk_gemm_bf16(int epi, int a_mn_major, int b_mn_major, const void* A, long l
 int ofk_gemm_reserve_sms(int n);
 
 /* Same GEMM with grouped row maps (logical row r -> (r / rows_per_group) * group_stride + group_offset + r % rpg):
- *   out_*  : where the rows of `out` go inside a larger interleaved buffer (STORE_BF16 / BIAS_BF16 / STORE_F32);
+ *   out_*  : where the rows of `out` go inside a larger interleaved buffer (STORE_BF16 / BIAS_BF16 / STORE_F32;
+ *            M must be a multiple of rows_per_group, else OFK_ERR_ARG);
  *   a_k_*  : which physical rows of an MN-major A form the reduction dimension (rows_per_group % 64 == 0).
  * Lets PerceiverAttention's k/v for the media tokens and for the latents (helpers.py:53-54: to_kv(cat(x, latents)))
  * be produced by two GEMMs that write straight into the concatenated [b*T, v+n, 2*inner] layout, and lets the

@@ -62,13 +62,20 @@ struct GemmParams {
   long long ldaux;
   const float* bias;
   const float* gate;
-  int stream_out;    // 1: epilogue outputs use st.global.cs (evict-first) so they do not displace the operand panels in L2
+  int stream_out;    // 1: epilogue stores carry an L2 evict-first hint so they do not displace the operand panels in L2
   // Grouped row maps (0 = identity): logical row r -> (r / rpg) * gs + go + r % rpg.  `out_*` places the rows of `out`
   // inside a larger interleaved buffer (the media / latent halves of PerceiverAttention's cat((x, latents), -2),
   // helpers.py:53); `ak_*` does the same for the REDUCTION rows of an MN-major A operand (wgrad over one half).
   int out_rpg, out_gs, out_go;
   int ak_rpg, ak_gs, ak_go;
   int wide;          // 1: 128 x 256 tiles on 2-CTA clusters sharing B (launched with a cluster); 0: 128 x 128 tiles
+  // Set by launch() for the chosen shape.  Read from the parameter bank rather than derived in the kernel, so they
+  // take no registers through the main loop and the epilogue.
+  int m_units;       // m-tiles (narrow) or m-tile pairs (wide)
+  int n_tiles;
+  int num_work;      // m_units * n_tiles * splits
+  int total_kb;      // k-blocks of K
+  int out_chunk;     // grouped out map: rows per TMA store (a box never crosses a group)
 };
 __device__ __forceinline__ long long map_rows(long long r, int rpg, int gs, int go) {
   return rpg > 0 ? (r / rpg) * gs + go + r % rpg : r;
@@ -91,187 +98,106 @@ __device__ __forceinline__ void work_to_tile(int w, int m_tiles, int n_tiles, in
 }
 
 // ----------------------------------------------------------------------------------------------
-// Epilogue.  One warp drains 32 accumulator rows (lane = row) x 32 columns per round.  A lane owns a ROW, so a
-// naive "each lane stores its row" epilogue issues warp stores that touch 32 different cache lines.
-// Instead every global access goes through a per-warp shared-memory staging tile and is re-issued TRANSPOSED:
-// consecutive lanes touch consecutive 16-byte pieces of the same row (4 or 8 rows per instruction), i.e. full
-// 64/128-byte segments.  The same staging tile is used for the epilogue's reads (residual, saved pre-activation).
-constexpr int STAGE_ROW = 128;                     // unpadded 128 B rows; the 16-byte piece index is XOR-swizzled with
-constexpr int STAGE_BYTES_PER_WARP = 32 * STAGE_ROW;   // (row & 7) so row-wise and piece-wise accesses are conflict-free
-__device__ __forceinline__ uint32_t stage_off(int row, int piece) { return (uint32_t)(row * STAGE_ROW + ((piece ^ (row & 7)) << 4)); }
+// Epilogue.  Each consumer warpgroup finishes its 64 rows of the tile in sub-tiles of SUBN columns, straight from the
+// wgmma accumulator fragments: the fused arithmetic runs in registers, the results go to an epilogue buffer in shared
+// memory laid out as one box of the output's tensor map (64 rows x SUBN columns, TMA-swizzled), and one thread of the
+// warpgroup writes the box with an asynchronous TMA store (a TMA reduce-add for ATOMIC_F32).  The aux operand (fp32
+// residual, bf16 saved pre-activation) is TMA-loaded into the sub-tile's out buffer NBUF - 1 sub-tiles ahead (across
+// the tile boundary into the next tile's first sub-tiles, so those loads overlap its main loop), and the result
+// overwrites it in place.  A sub-tile's aux load completes before its store is issued, so an in-place residual
+// (aux == out) is exact.  out2 has buffers of its own.
+template <int EPI>
+struct EpiTraits {
+  static constexpr bool RESID = EPI == OFK_EPI_GATE_RESID_F32 || EPI == OFK_EPI_BIAS_RESID_F32;
+  static constexpr bool F32_OUT = RESID || EPI == OFK_EPI_STORE_F32 || EPI == OFK_EPI_ATOMIC_F32;
+  static constexpr bool HAS_OUT2 = RESID || EPI == OFK_EPI_GELU_DUAL;
+  static constexpr bool HAS_BIAS = EPI == OFK_EPI_BIAS_BF16 || EPI == OFK_EPI_BIAS_QGELU_BF16 ||
+                                   EPI == OFK_EPI_BIAS_GELU_BF16 || EPI == OFK_EPI_BIAS_RESID_F32;
+  static constexpr int AUX_BYTES = RESID ? 4 : (EPI == OFK_EPI_DGELU_BF16 ? 2 : 0);
+  static constexpr int OUT_BYTES = F32_OUT ? 4 : 2;
+  // Columns per sub-tile and buffers per warpgroup, within 16 KiB: one-output epilogues use 128-byte box rows (one
+  // 128-byte swizzle span, conflict-free fragment writes) double-buffered; GELU_DUAL two bf16 32-column boxes, each
+  // double-buffered; DGELU a 32-column bf16 box four deep (its aux load runs three sub-tiles ahead); the residual
+  // epilogues, the heaviest, 16 columns: fp32 out with the aux in place three deep (4 KiB each; the residual load runs
+  // two sub-tiles ahead) and bf16 out2 double-buffered (2 KiB each).
+  static constexpr int SUBN = RESID ? 16 : (EPI == OFK_EPI_GELU_DUAL || EPI == OFK_EPI_DGELU_BF16) ? 32 : 128 / OUT_BYTES;
+  static constexpr int NBUF = EPI == OFK_EPI_DGELU_BF16 ? 4 : RESID ? 3 : 2;   // out (and aux) buffers
+  static constexpr int NBUF2 = HAS_OUT2 ? 2 : 0;                                 // out2 buffers
+  static constexpr int OUT_PITCH = SUBN * OUT_BYTES;    // bytes per box row = the map's swizzle span (32, 64 or 128)
+  static constexpr int OUT2_PITCH = SUBN * 2;
+  static constexpr int OUT_BUF_BYTES = 64 * OUT_PITCH;
+  static constexpr int OUT2_BUF_BYTES = 64 * OUT2_PITCH;
+  static constexpr int OUT2_BASE = NBUF * OUT_BUF_BYTES;
+  static constexpr int BYTES = OUT2_BASE + NBUF2 * OUT2_BUF_BYTES;
+  static_assert(OUT_BUF_BYTES % 1024 == 0 && OUT2_BUF_BYTES % 1024 == 0, "boxes start on a swizzle-pattern boundary");
+  // Before a sub-tile's barrier the issuing thread lets at most PRE_WAIT stores still read their buffers, so the next
+  // sub-tile's out2 buffer (and, without an aux load to wait on, its out buffer) is free after the barrier; -1: no wait
+  // (an aux epilogue's out buffer is refilled only after its store has read it, see the consumer).
+  static constexpr int PRE_WAIT = AUX_BYTES != 0 ? (HAS_OUT2 ? NBUF2 - 2 : -1)
+                                                 : (HAS_OUT2 && NBUF2 < NBUF ? NBUF2 - 2 : NBUF - 2);
+};
 
-
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint4 v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+// Byte offset of (row, byte column) in a box with PITCH-byte rows, swizzled as the map's CU_TENSOR_MAP_SWIZZLE_<PITCH>B
+// does it: the 16-byte chunk index is XORed with address bits [7, 7 + log2(PITCH / 16)) (boxes are 1024-byte aligned).
+template <int PITCH>
+__device__ __forceinline__ int box_off(int row, int byte_col) {
+  return row * PITCH + ((((byte_col >> 4) ^ ((row * PITCH) >> 7)) & (PITCH / 16 - 1)) << 4) + (byte_col & 15);
 }
-__device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_b32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_shared_f32x2(uint32_t addr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ float2 ld_shared_f32x2(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
   return v;
 }
 
-// Store this warp's 32 x 32 tile (lane's row in `w`: WORDS = 32 for f32, 16 for bf16) to global, coalesced.
-// MODE 0 = plain store, 1 = red.global.add.f32 (f32 only).
-__device__ __forceinline__ void st_global_cs_v4(void* g, uint4 v) {
-  asm volatile("st.global.cs.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(g), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-
-template <int ELEM_BYTES, int MODE>
-__device__ __forceinline__ void warp_store_tile(uint32_t stage, const uint32_t* w, void* gbase, long long ld, int row0,
-                                                int col0, int M, int N, int streaming = 0, int rpg = 0, int gs = 0,
-                                                int go = 0) {
-  constexpr int PIECES = ELEM_BYTES * 2;            // 16-byte pieces per 32-element row: 8 (f32) or 4 (bf16)
-  constexpr int EPP = 16 / ELEM_BYTES;              // elements per piece
-  const int lane = threadIdx.x & 31;
-#pragma unroll
-  for (int i = 0; i < PIECES; ++i)
-    st_shared_v4(stage + stage_off(lane, i), make_uint4(w[4 * i], w[4 * i + 1], w[4 * i + 2], w[4 * i + 3]));
-  __syncwarp();
-  const int piece = lane % PIECES, rsub = lane / PIECES;
-  const int col = col0 + piece * EPP;
-#pragma unroll
-  for (int it = 0; it < PIECES; ++it) {
-    const int r = it * (32 / PIECES) + rsub;
-    const uint4 v = ld_shared_v4(stage + stage_off(r, piece));
-    const int row = row0 + r;
-    if (row < M && col < N) {
-      uint8_t* g = reinterpret_cast<uint8_t*>(gbase) + (map_rows(row, rpg, gs, go) * ld + col) * ELEM_BYTES;
-      if constexpr (MODE == 0) {
-        if (streaming) st_global_cs_v4(g, v);
-        else *reinterpret_cast<uint4*>(g) = v;
-      } else {
-        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(g), "f"(__uint_as_float(v.x)),
-                     "f"(__uint_as_float(v.y)), "f"(__uint_as_float(v.z)), "f"(__uint_as_float(v.w))
-                     : "memory");
-      }
-    }
-  }
-  __syncwarp();
-}
-
-// Epilogue operand (residual / saved pre-activation) tile, two-phase so the global latency is hidden:
-//   aux_prefetch: coalesced global loads of this warp's 32 x 32 tile into registers (issued one round ahead)
-//   aux_commit  : registers -> staging tile -> each lane reads its own row
-template <int ELEM_BYTES>
-__device__ __forceinline__ void aux_prefetch(uint4 (&pre)[ELEM_BYTES * 2], const void* gbase, long long ld, int row0,
-                                             int col0, int M, int N) {
-  constexpr int PIECES = ELEM_BYTES * 2;
-  constexpr int EPP = 16 / ELEM_BYTES;
-  const int lane = threadIdx.x & 31;
-  const int piece = lane % PIECES, rsub = lane / PIECES;
-  const int col = col0 + piece * EPP;
-#pragma unroll
-  for (int it = 0; it < PIECES; ++it) {
-    const int row = row0 + it * (32 / PIECES) + rsub;
-    pre[it] = make_uint4(0u, 0u, 0u, 0u);
-    if (row < M && col < N)
-      pre[it] = *reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(gbase) + ((long long)row * ld + col) * ELEM_BYTES);
-  }
-}
-template <int ELEM_BYTES>
-__device__ __forceinline__ void aux_commit(uint32_t stage, const uint4 (&pre)[ELEM_BYTES * 2], uint32_t* w) {
-  constexpr int PIECES = ELEM_BYTES * 2;
-  const int lane = threadIdx.x & 31;
-  const int piece = lane % PIECES, rsub = lane / PIECES;
-#pragma unroll
-  for (int it = 0; it < PIECES; ++it) st_shared_v4(stage + stage_off(it * (32 / PIECES) + rsub, piece), pre[it]);
-  __syncwarp();
-#pragma unroll
-  for (int i = 0; i < PIECES; ++i) {
-    const uint4 v = ld_shared_v4(stage + stage_off(lane, i));
-    w[4 * i] = v.x; w[4 * i + 1] = v.y; w[4 * i + 2] = v.z; w[4 * i + 3] = v.w;
-  }
-  __syncwarp();
-}
-
+// The fused epilogue of two adjacent accumulators, columns (c, c + 1) of row r of the sub-tile whose out / out2
+// buffers are at shared addresses `buf` / `buf2` (c even); bias already added.  The operations and their rounding
+// points are the same for every element wherever it sits.
 template <int EPI>
-struct AuxBytes { static constexpr int value = (EPI == OFK_EPI_GATE_RESID_F32 || EPI == OFK_EPI_BIAS_RESID_F32) ? 4 : (EPI == OFK_EPI_DGELU_BF16 ? 2 : 0); };
-
-__device__ __forceinline__ void pack32_bf16(const float (&v)[32], uint32_t (&w)[16]) {
-#pragma unroll
-  for (int i = 0; i < 16; ++i) w[i] = pack_bf16x2(v[2 * i], v[2 * i + 1]);
-}
-
-// One round: rows [row0, row0+32) (lane = row) x columns [col0, col0+32), accumulators in `acc`.
-template <int EPI>
-__device__ __forceinline__ void epilogue32(const GemmParams& p, float gate_t, uint32_t stage, int row0, int col0,
-                                           const uint32_t (&acc)[32], uint32_t* aux_row) {
-  float v[32];
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(acc[i]);
-  constexpr bool HAS_BIAS = EPI == OFK_EPI_BIAS_BF16 || EPI == OFK_EPI_BIAS_QGELU_BF16 || EPI == OFK_EPI_BIAS_GELU_BF16 ||
-                            EPI == OFK_EPI_BIAS_RESID_F32;
-  if constexpr (HAS_BIAS) {
-    // every lane needs the same 32 bias values: broadcast loads (one wavefront each)
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      if (col0 + 4 * i < p.N) {
-        const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + col0) + i);
-        v[4 * i] += b.x; v[4 * i + 1] += b.y; v[4 * i + 2] += b.z; v[4 * i + 3] += b.w;
-      }
-    }
-  }
-
+__device__ __forceinline__ void epilogue_pair(const GemmParams& p, float gate_t, uint32_t buf, uint32_t buf2, int r,
+                                              int c, float v0, float v1) {
+  using E = EpiTraits<EPI>;
+  const uint32_t o = buf + box_off<E::OUT_PITCH>(r, c * E::OUT_BYTES);
+  const uint32_t o2 = buf2 + box_off<E::OUT2_PITCH>(r, c * 2);
   if constexpr (EPI == OFK_EPI_STORE_BF16 || EPI == OFK_EPI_BIAS_BF16 || EPI == OFK_EPI_BIAS_QGELU_BF16 ||
                 EPI == OFK_EPI_BIAS_GELU_BF16) {
-    if constexpr (EPI == OFK_EPI_BIAS_QGELU_BF16) {
-#pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = quick_gelu(bf16_round(v[i]));
-    }
-    if constexpr (EPI == OFK_EPI_BIAS_GELU_BF16) {
-#pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = gelu_exact(bf16_round(v[i]));
-    }
-    uint32_t w[16];
-    pack32_bf16(v, w);
-    warp_store_tile<2, 0>(stage, w, p.out, p.ldo, row0, col0, p.M, p.N, p.stream_out, p.out_rpg, p.out_gs, p.out_go);
-  } else if constexpr (EPI == OFK_EPI_STORE_F32) {
-    warp_store_tile<4, 0>(stage, acc, p.out, p.ldo, row0, col0, p.M, p.N, p.stream_out, p.out_rpg, p.out_gs, p.out_go);
-  } else if constexpr (EPI == OFK_EPI_ATOMIC_F32) {
-    warp_store_tile<4, 1>(stage, acc, p.out, p.ldo, row0, col0, p.M, p.N);
+    if constexpr (EPI == OFK_EPI_BIAS_QGELU_BF16) { v0 = quick_gelu(bf16_round(v0)); v1 = quick_gelu(bf16_round(v1)); }
+    if constexpr (EPI == OFK_EPI_BIAS_GELU_BF16) { v0 = gelu_exact(bf16_round(v0)); v1 = gelu_exact(bf16_round(v1)); }
+    st_shared_b32(o, pack_bf16x2(v0, v1));
+  } else if constexpr (EPI == OFK_EPI_STORE_F32 || EPI == OFK_EPI_ATOMIC_F32) {
+    st_shared_f32x2(o, v0, v1);
   } else if constexpr (EPI == OFK_EPI_GELU_DUAL) {
     // z = bf16(acc) is what the reference's Linear emits under autocast; GELU is taken of that.
-    uint32_t wz[16], wh[16];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = bf16_round(v[i]);
-    pack32_bf16(v, wz);
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = gelu_exact(v[i]);
-    pack32_bf16(v, wh);
-    warp_store_tile<2, 0>(stage, wz, p.out, p.ldo, row0, col0, p.M, p.N, p.stream_out);
-    warp_store_tile<2, 0>(stage, wh, p.out2, p.ldo2, row0, col0, p.M, p.N, p.stream_out);
-  } else if constexpr (EPI == OFK_EPI_GATE_RESID_F32 || EPI == OFK_EPI_BIAS_RESID_F32) {
+    v0 = bf16_round(v0); v1 = bf16_round(v1);
+    st_shared_b32(o, pack_bf16x2(v0, v1));
+    st_shared_b32(o2, pack_bf16x2(gelu_exact(v0), gelu_exact(v1)));
+  } else if constexpr (E::RESID) {
     // out = branch * tanh(gate) + residual (fp32 residual stream); branch kept in bf16 for the gate grad.
-    uint32_t* r = aux_row;   // this lane's 32 residual values (prefetched one round ahead)
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = bf16_round(v[i]);
-    if (p.out2 != nullptr) {
-      uint32_t wb[16];
-      pack32_bf16(v, wb);
-      warp_store_tile<2, 0>(stage, wb, p.out2, p.ldo2, row0, col0, p.M, p.N, p.stream_out);
-    }
-#pragma unroll
-    for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(fmaf(v[i], gate_t, __uint_as_float(r[i])));
-    warp_store_tile<4, 0>(stage, r, p.out, p.ldo, row0, col0, p.M, p.N, p.stream_out);
+    v0 = bf16_round(v0); v1 = bf16_round(v1);
+    if (p.out2 != nullptr) st_shared_b32(o2, pack_bf16x2(v0, v1));
+    const float2 res = ld_shared_f32x2(o);
+    st_shared_f32x2(o, fmaf(v0, gate_t, res.x), fmaf(v1, gate_t, res.y));
   } else if constexpr (EPI == OFK_EPI_DGELU_BF16) {
     // out = bf16( bf16(acc) * gelu'(z) ), z = saved bf16 pre-activation
-    uint32_t w[16];
-    const uint32_t* z = aux_row;
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      v[2 * i] = bf16_round(v[2 * i]) * gelu_exact_grad(bf16_lo(z[i]));
-      v[2 * i + 1] = bf16_round(v[2 * i + 1]) * gelu_exact_grad(bf16_hi(z[i]));
-    }
-    pack32_bf16(v, w);
-    warp_store_tile<2, 0>(stage, w, p.out, p.ldo, row0, col0, p.M, p.N, p.stream_out, p.out_rpg, p.out_gs, p.out_go);
+    const uint32_t z = ld_shared_b32(o);
+    st_shared_b32(o, pack_bf16x2(bf16_round(v0) * gelu_exact_grad(bf16_lo(z)), bf16_round(v1) * gelu_exact_grad(bf16_hi(z))));
   }
 }
 
 // ----------------------------------------------------------------------------------------------
-// Shared memory: the TMA ring of 4 stages (a stage holds A, then B), then the per-warp epilogue staging tiles.
-// The epilogue moves accumulator fragments through 64 x 64 fp32 slabs (one per consumer warpgroup), re-read lane = row:
-//   narrow: one slab pair, in the ring space the 32 KiB stages leave free;
-//   wide  : the tile's last 4 ring stages, one per quarter of the columns (see the consumer).
+// Shared memory: the TMA ring of 4 stages (a stage holds A, then B), then the epilogue buffers (16 KiB per consumer
+// warpgroup), then the barriers.
 struct SmemLayout {
   static constexpr int A_BYTES = BM * BK * 2;                        // 16 KiB
   static constexpr int B_PART_BYTES = BN * BK * 2;                   // 16 KiB: the B rows one CTA loads
@@ -279,34 +205,23 @@ struct SmemLayout {
   static constexpr int WIDE_STAGE_BYTES = A_BYTES + CLUSTER * B_PART_BYTES;   // 48 KiB
   static constexpr int STAGES = 4;
   static constexpr int RING_BYTES = STAGES * WIDE_STAGE_BYTES;
-  static constexpr int ACC_PITCH = 64 + 8;      // floats; 8 mod 32 keeps the fragment stores conflict-free
-  static constexpr int ACC_BYTES = 64 * ACC_PITCH * 4;
-  static constexpr int ACC_OFF = STAGES * NARROW_STAGE_BYTES;   // narrow only
-  static_assert(ACC_OFF + NUM_CONSUMER_WG * ACC_BYTES <= RING_BYTES, "the narrow slabs fit beside the narrow ring");
-  static_assert(NUM_CONSUMER_WG * ACC_BYTES <= WIDE_STAGE_BYTES, "a parked quarter fits a wide stage");
   static constexpr int EPI_OFF = RING_BYTES;
-  static constexpr int BAR_OFF = EPI_OFF + NUM_EPI_WARPS * STAGE_BYTES_PER_WARP;
+  static constexpr int EPI_BYTES_PER_WG = 16 * 1024;
+  static constexpr int MAX_NBUF = 4;
+  static constexpr int BAR_OFF = EPI_OFF + NUM_CONSUMER_WG * EPI_BYTES_PER_WG;
+  static constexpr int NUM_BARS = 2 * STAGES + NUM_CONSUMER_WG * MAX_NBUF;   // full, empty, aux per warpgroup
   static constexpr int TOTAL = BAR_OFF + 256 + 1024;   // + barriers + alignment slack
+  static_assert(NUM_BARS * 8 <= 256, "barriers fit their region");
 };
 static_assert(SmemLayout::TOTAL <= 227 * 1024, "GEMM shared memory exceeds the sm_90 per-block limit");
-
-// Accumulator fragments of columns [64 h, 64 h + 64) -> a 64 x 64 fp32 slab (pitch ACC_PITCH), for lane = row re-reads.
-template <int NACC>
-__device__ __forceinline__ void park_part(float* slab, const float (&d)[NACC], int h, int wl, int lane) {
-  const int fr = 16 * wl + lane / 4, fc = 2 * (lane % 4);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const int i = 4 * (8 * h + j);
-    *reinterpret_cast<float2*>(slab + fr * SmemLayout::ACC_PITCH + 8 * j + fc) = make_float2(d[i], d[i + 1]);
-    *reinterpret_cast<float2*>(slab + (fr + 8) * SmemLayout::ACC_PITCH + 8 * j + fc) = make_float2(d[i + 2], d[i + 3]);
-  }
-}
 
 template <int A_MN, int B_MN, int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
-            const GemmParams p) {
+            const __grid_constant__ CUtensorMap tma_out, const __grid_constant__ CUtensorMap tma_out2,
+            const __grid_constant__ CUtensorMap tma_aux, const GemmParams p) {
   using L = SmemLayout;
+  using E = EpiTraits<EPI>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
@@ -318,28 +233,28 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
   // Wide: the CTAs of a cluster walk the work items together (consecutive blockIdx.x form a cluster); CTA `crank`
   // takes m-tile 2 * unit + crank and loads B rows [128 crank, 128 crank + 128) of the tile for both.  When the
   // m-tile count is odd, the last pair's second tile lies wholly past M: it still loads (TMA fills zeros) and
-  // arrives, and its stores are masked by row < M.
+  // arrives, and its stores fall outside the output map, so TMA writes nothing.
   const bool wide = p.wide != 0;
   const int bn = wide ? BN_WIDE : BN;
   const int stage_bytes = wide ? L::WIDE_STAGE_BYTES : L::NARROW_STAGE_BYTES;
   const int crank = wide ? (int)cluster_ctarank() : 0;
   const int walker = wide ? blockIdx.x / CLUSTER : blockIdx.x;
   const int walkers = wide ? gridDim.x / CLUSTER : gridDim.x;
-  const int m_tiles = (p.M + BM - 1) / BM;
-  const int m_units = wide ? (m_tiles + 1) / 2 : m_tiles;
-  const int n_tiles = (p.N + bn - 1) / bn;
-  const int num_work = m_units * n_tiles * p.splits;
-  const int total_kb = (p.K + BK - 1) / BK;
+  const int m_units = p.m_units, n_tiles = p.n_tiles, num_work = p.num_work, total_kb = p.total_kb;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
+    tma_prefetch_desc(&tma_out);
+    if constexpr (E::HAS_OUT2) tma_prefetch_desc(&tma_out2);
+    if constexpr (E::AUX_BYTES != 0) tma_prefetch_desc(&tma_aux);
     // wide: a stage is freed only when the consumers of BOTH CTAs are done with it, since the partner's producer
     // multicasts into this CTA's copy of the stage
     for (int s = 0; s < L::STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], NUM_EPI_WARPS * (wide ? CLUSTER : 1));
     }
+    for (int b = 0; b < NUM_CONSUMER_WG * L::MAX_NBUF; ++b) mbar_init(&full_bar[2 * L::STAGES + b], 1);
     fence_barrier_init();
   }
   // wide: the partner's barriers must be initialised before anything is multicast or arrived on them
@@ -396,9 +311,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
   const int wg = warp / 4 - 1;               // consumer warpgroup: accumulator rows [64 wg, 64 wg + 64) of the tile
   const int wl = warp & 3;                   // warp within the warpgroup
-  const int epi_warp = warp - 4;
-  float* acc_slab = reinterpret_cast<float*>(smem + L::ACC_OFF + wg * L::ACC_BYTES);
-  const uint32_t stage_addr = smem_u32(smem + L::EPI_OFF) + epi_warp * STAGE_BYTES_PER_WARP;
+  const bool leader = (threadIdx.x & 127) == 0;   // issues the warpgroup's epilogue TMA stores and aux loads
+  uint8_t* ebuf = smem + L::EPI_OFF + wg * L::EPI_BYTES_PER_WG;
+  uint64_t* aux_bar = full_bar + 2 * L::STAGES + wg * L::MAX_NBUF;
   float gate_t = 1.0f;
   if constexpr (EPI == OFK_EPI_GATE_RESID_F32) {
     if (p.gate != nullptr) gate_t = tanhf(__ldg(p.gate));
@@ -408,6 +323,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
     constexpr bool WIDE = decltype(wide_c)::value;
     constexpr int TILE_N = WIDE ? BN_WIDE : BN;
     constexpr int STAGE_BYTES = WIDE ? L::WIDE_STAGE_BYTES : L::NARROW_STAGE_BYTES;
+    constexpr int SUBN = E::SUBN, NBUF = E::NBUF, SUBT = TILE_N / SUBN;
+    static_assert(E::BYTES <= L::EPI_BYTES_PER_WG && NBUF <= L::MAX_NBUF && NBUF - 1 < SUBT, "epilogue buffers");
     auto release = [&](int s) {
       if (lane != 0) return;
       if constexpr (WIDE) {
@@ -417,12 +334,72 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
         mbar_arrive(&empty_bar[s]);
       }
     };
+    // This warpgroup's first row and the tile's first column for work item w.
+    auto tile_origin = [&](int w, int& row0, int& col0) {
+      int mu, nt, ks;
+      work_to_tile(w, m_units, n_tiles, mu, nt, ks);
+      row0 = (WIDE ? 2 * mu + crank : mu) * BM + wg * 64;
+      col0 = nt * TILE_N;
+    };
+    // Leader only: TMA-load the aux box at (row0, col) for the q-th sub-tile of this warpgroup.
+    auto load_aux = [&](uint32_t q, int row0, int col) {
+      uint64_t* bar = &aux_bar[q % NBUF];
+      mbar_arrive_expect_tx(bar, 64 * SUBN * E::AUX_BYTES);
+      tma_load_2d(ebuf + (q % NBUF) * E::OUT_BUF_BYTES, &tma_aux, bar, col, row0);
+    };
+    // ... for sub-tile s of work item w, if there is one
+    auto load_aux_of = [&](uint32_t q, int w, int s) {
+      if (w >= num_work) return;
+      int row0, col0;
+      tile_origin(w, row0, col0);
+      load_aux(q, row0, col0 + s * SUBN);
+    };
+    // Leader only: store the sub-tile at (row0, col).  A grouped output map is a 3-D map (columns, rows in group,
+    // groups) whose box is p.out_chunk rows that never cross a group (see gemm_impl): the 64 rows go out in
+    // 64 / out_chunk stores, each at non-negative coordinates, and those wholly past M are skipped.
+    auto store_out = [&](const uint8_t* buf, const uint8_t* buf2, int row0, int col) {
+      constexpr bool GROUPED = EPI == OFK_EPI_STORE_BF16 || EPI == OFK_EPI_BIAS_BF16 || EPI == OFK_EPI_STORE_F32;
+      static_assert(!GROUPED || E::OUT_PITCH == 128, "a grouped store starts at any row: rows must be 128-byte aligned");
+      const uint64_t policy = p.stream_out ? l2_policy_evict_first() : 0;
+      if constexpr (EPI == OFK_EPI_ATOMIC_F32) {
+        tma_reduce_add_3d(&tma_out, buf, col, row0, 0);
+      } else if constexpr (GROUPED) {
+        if (p.out_rpg == 0) {
+          if (p.stream_out) tma_store_3d_hint(&tma_out, buf, col, row0, 0, policy);
+          else tma_store_3d(&tma_out, buf, col, row0, 0);
+        } else {
+          for (int r = row0; r < row0 + 64 && r < p.M; r += p.out_chunk) {
+            const uint8_t* src = buf + (r - row0) * E::OUT_PITCH;
+            const int g = r / p.out_rpg;
+            if (p.stream_out) tma_store_3d_hint(&tma_out, src, col, r - g * p.out_rpg, g, policy);
+            else tma_store_3d(&tma_out, src, col, r - g * p.out_rpg, g);
+          }
+        }
+      } else {
+        if (p.stream_out) tma_store_3d_hint(&tma_out, buf, col, row0, 0, policy);
+        else tma_store_3d(&tma_out, buf, col, row0, 0);
+      }
+      if constexpr (E::HAS_OUT2) {
+        if (p.out2 != nullptr) {
+          if (p.stream_out) tma_store_2d_hint(&tma_out2, buf2, col, row0, policy);
+          else tma_store_2d(&tma_out2, buf2, col, row0);
+        }
+      }
+      bulk_commit_group();
+    };
+
     int stage = 0; uint32_t phase = 0;
+    uint32_t q = 0;   // sub-tiles this warpgroup has finished
+    if constexpr (E::AUX_BYTES != 0) {
+      if (leader) {
+#pragma unroll
+        for (int s = 0; s < NBUF - 1; ++s) load_aux_of(s, walker, s);
+      }
+    }
     float d[TILE_N / 2];
     for (int w = walker; w < num_work; w += walkers) {
       int mu, nt, ks;
       work_to_tile(w, m_units, n_tiles, mu, nt, ks);
-      const int mt = WIDE ? 2 * mu + crank : mu;
       const int kb0 = ks * p.kb_per_split;
       const int kb1 = min(total_kb, kb0 + p.kb_per_split);
       // The first k-step overwrites the accumulators (scale-d = 0), but wgmma still names them as inputs: zeroing them
@@ -454,68 +431,64 @@ gemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ C
         wgmma_commit();
         // keep one k-block of MMAs in flight; the one before it has retired, so its ring slot can be refilled
         wgmma_wait<1>();
-        // wide: the stages of the tile's last STAGES k-blocks are kept for the epilogue
-        if (prev_stage >= 0 && !(WIDE && kb > kb1 - L::STAGES)) release(prev_stage);
+        if (prev_stage >= 0) release(prev_stage);
         prev_stage = stage;
         if (++stage == L::STAGES) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
+      // every stage goes back to the producer before the epilogue, so the next tile's loads overlap it
+      release(prev_stage);
 
-      // Epilogue, in parts of 64 columns: fragments -> a 64 x 64 slab, then each warp re-reads one 32 x 32 block with
-      // lane = row and runs the shared fused epilogue on it.
-      const int rh = wl & 1, ch = wl >> 1;
-      const int row0 = mt * BM + wg * 64 + rh * 32;
-      constexpr int AUXB = AuxBytes<EPI>::value;
-      auto run_part = [&](const float* slab, int col0) {
-        uint32_t acc[32];
-        const float* src = slab + (rh * 32 + lane) * L::ACC_PITCH + ch * 32;
+      // Epilogue, one sub-tile of SUBN columns at a time, from the live fragments: thread t of the warpgroup holds
+      // rows fr and fr + 8 of the 64, columns 8 j + fc and 8 j + fc + 1 of every 8 (wgmma_m64n128k16_bf16's layout).
+      int row0, col0;
+      tile_origin(w, row0, col0);
+      const int fr = 16 * wl + lane / 4, fc = 2 * (lane % 4);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 v = *reinterpret_cast<const float4*>(src + 4 * i);
-          acc[4 * i] = __float_as_uint(v.x); acc[4 * i + 1] = __float_as_uint(v.y);
-          acc[4 * i + 2] = __float_as_uint(v.z); acc[4 * i + 3] = __float_as_uint(v.w);
-        }
-        const int col = col0 + ch * 32;
-        if (row0 < p.M && col < p.N) {                                                 // warp-uniform
-          uint32_t aux_row[AUXB ? AUXB * 8 : 1];
-          if constexpr (AUXB != 0) {
-            uint4 pre[AUXB * 2];
-            aux_prefetch<AUXB>(pre, p.aux, p.ldaux, row0, col, p.M, p.N);
-            aux_commit<AUXB>(stage_addr, pre, aux_row);
+      for (int s = 0; s < SUBT; ++s) {
+        const uint32_t qs = q + s;
+        uint8_t* buf = ebuf + (qs % NBUF) * E::OUT_BUF_BYTES;
+        uint8_t* buf2 = ebuf + E::OUT2_BASE + (qs % (E::NBUF2 > 0 ? E::NBUF2 : 1)) * E::OUT2_BUF_BYTES;
+        const uint32_t sbuf = smem_u32(buf), sbuf2 = smem_u32(buf2);
+        if constexpr (E::AUX_BYTES != 0) mbar_wait(&aux_bar[qs % NBUF], (qs / NBUF) & 1);
+#pragma unroll
+        for (int j = 0; j < SUBN / 8; ++j) {
+          const int c = 8 * j + fc;
+          const int i = 4 * (s * (SUBN / 8) + j);
+          float b0 = 0.f, b1 = 0.f;
+          if constexpr (E::HAS_BIAS) {
+            // per-column bias: the four lanes of a row read 8 consecutive floats, every row the same (broadcast)
+            if (col0 + s * SUBN + c < p.N) {
+              const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + s * SUBN + c));
+              b0 = b.x; b1 = b.y;
+            }
           }
-          epilogue32<EPI>(p, gate_t, stage_addr, row0, col, acc, aux_row);
+          epilogue_pair<EPI>(p, gate_t, sbuf, sbuf2, fr, c, E::HAS_BIAS ? d[i] + b0 : d[i],
+                             E::HAS_BIAS ? d[i + 1] + b1 : d[i + 1]);
+          epilogue_pair<EPI>(p, gate_t, sbuf, sbuf2, fr + 8, c, E::HAS_BIAS ? d[i + 2] + b0 : d[i + 2],
+                             E::HAS_BIAS ? d[i + 3] + b1 : d[i + 3]);
         }
-      };
-      if constexpr (!WIDE) {
-        release(prev_stage);
-#pragma unroll
-        for (int h = 0; h < BN / 64; ++h) {
-          named_bar_sync(1 + wg, 128);         // the previous part's readers are done with the slab
-          park_part(acc_slab, d, h, wl, lane);
-          named_bar_sync(1 + wg, 128);
-          run_part(acc_slab, nt * BN + h * 64);
+        // the TMA store (async proxy) must see these generic-proxy writes
+        fence_proxy_async_smem();
+        // the next sub-tile's buffers without an aux load to wait on are free once the stores that last read them have
+        if constexpr (E::PRE_WAIT >= 0) {
+          if (leader) bulk_wait_group_read<E::PRE_WAIT>();
         }
-      } else {
-        // The kernel has 168 registers per thread; 128 live accumulators would leave the epilogue too few.  So all four
-        // quarters leave the registers first, into the ring stages of the tile's last four k-blocks (a wide tile has
-        // at least STAGES k-blocks), each returned to the producer once its quarter has been read.  Both warpgroups
-        // must be done with those stages' operands.
-        named_bar_sync(1 + NUM_CONSUMER_WG, 128 * NUM_CONSUMER_WG);
-        auto part_stage = [&](int h) { return (prev_stage + 1 + h) % L::STAGES; };   // h = 3: the last k-block's
-        auto part = [&](int h) { return reinterpret_cast<float*>(smem + part_stage(h) * STAGE_BYTES + wg * L::ACC_BYTES); };
-#pragma unroll
-        for (int h = 0; h < BN_WIDE / 64; ++h) park_part(part(h), d, h, wl, lane);
         named_bar_sync(1 + wg, 128);
-#pragma unroll 1
-        for (int h = 0; h < BN_WIDE / 64; ++h) {
-          run_part(part(h), nt * BN_WIDE + h * 64);
-          // the TMA (async proxy) refill of the stage must not overtake these generic-proxy accesses
-          fence_proxy_async_smem();
-          __syncwarp();
-          release(part_stage(h));
+        if (leader) {
+          store_out(buf, buf2, row0, col0 + s * SUBN);
+          if constexpr (E::AUX_BYTES != 0) {
+            // the buffer of sub-tile qs - 1 is free once its store has read it: load sub-tile qs + NBUF - 1 into it
+            bulk_wait_group_read<1>();
+            if (s + NBUF - 1 < SUBT) load_aux(qs + NBUF - 1, row0, col0 + (s + NBUF - 1) * SUBN);
+            else load_aux_of(qs + NBUF - 1, w + walkers, s + NBUF - 1 - SUBT);
+          }
         }
       }
+      q += SUBT;
     }
+    // every bulk store must be complete before the CTA exits
+    if (leader) bulk_wait_group_all();
     // wide: neither CTA may exit while its partner can still arrive on its barriers (everything multicast into this
     // CTA has been consumed by now).  The cluster barrier waits for non-exited threads only: the producer warpgroup
     // has left.  (A barrier in the producer's code as well made ptxas hold the consumers to 168 registers, and spill.)
@@ -546,10 +519,11 @@ static EncodeTiledFn get_encode_fn() {
 }
 
 struct MapKey {
-  const void* ptr; long long ld; int rows, cols, box_inner, box_outer;
+  const void* ptr; long long ld, gstride; int rows, cols, groups, box_inner, box_outer, box_groups, elem_bytes, swizzle;
   bool operator==(const MapKey& o) const {
-    return ptr == o.ptr && ld == o.ld && rows == o.rows && cols == o.cols && box_inner == o.box_inner &&
-           box_outer == o.box_outer;
+    return ptr == o.ptr && ld == o.ld && gstride == o.gstride && rows == o.rows && cols == o.cols &&
+           groups == o.groups && box_inner == o.box_inner && box_outer == o.box_outer && box_groups == o.box_groups &&
+           elem_bytes == o.elem_bytes && swizzle == o.swizzle;
   }
 };
 struct MapKeyHash {
@@ -557,16 +531,21 @@ struct MapKeyHash {
     size_t h = reinterpret_cast<size_t>(k.ptr);
     h = h * 1000003u ^ (size_t)k.ld; h = h * 1000003u ^ (size_t)k.rows; h = h * 1000003u ^ (size_t)k.cols;
     h = h * 1000003u ^ (size_t)(k.box_inner * 1024 + k.box_outer);
+    h = h * 1000003u ^ (size_t)k.gstride; h = h * 1000003u ^ (size_t)(k.groups * 512 + k.box_groups);
+    h = h * 1000003u ^ (size_t)(k.elem_bytes * 1024 + k.swizzle);
     return h;
   }
 };
 
-// 2-D bf16 row-major tensor [rows, cols] (cols contiguous, row stride ld elements), 128B swizzle.
+// Row-major bf16 (elem_bytes 2) or fp32 (4) tensor [rows, cols] (cols contiguous, row stride ld elements), swizzled
+// in spans of `swizzle` bytes (32, 64 or 128).  groups = 0: 2-D, box {box_inner, box_outer}.  groups >= 1: 3-D
+// [groups, rows, cols] with a group stride of gstride elements, box {box_inner, box_outer, box_groups}.
 static int get_tensor_map(const void* ptr, long long ld, int rows, int cols, int box_inner, int box_outer,
-                          CUtensorMap* out) {
+                          CUtensorMap* out, int elem_bytes = 2, int swizzle = 128, int groups = 0,
+                          long long gstride = 0, int box_groups = 1) {
   static std::mutex mu;
   static std::unordered_map<MapKey, CUtensorMap, MapKeyHash> cache;
-  MapKey key{ptr, ld, rows, cols, box_inner, box_outer};
+  MapKey key{ptr, ld, gstride, rows, cols, groups, box_inner, box_outer, box_groups, elem_bytes, swizzle};
   {
     std::lock_guard<std::mutex> g(mu);
     auto it = cache.find(key);
@@ -574,18 +553,21 @@ static int get_tensor_map(const void* ptr, long long ld, int rows, int cols, int
   }
   EncodeTiledFn enc = get_encode_fn();
   if (!enc) return ofk_set_error(OFK_ERR_DRIVER, "cuTensorMapEncodeTiled entry point not found");
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {(cuuint32_t)box_inner, (cuuint32_t)box_outer};
-  cuuint32_t estr[2] = {1, 1};
+  const cuuint32_t rank = groups > 0 ? 3 : 2;
+  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)(groups > 0 ? groups : 1)};
+  cuuint64_t strides[2] = {(cuuint64_t)ld * elem_bytes, (cuuint64_t)gstride * elem_bytes};
+  cuuint32_t box[3] = {(cuuint32_t)box_inner, (cuuint32_t)box_outer, (cuuint32_t)box_groups};
+  cuuint32_t estr[3] = {1, 1, 1};
+  const CUtensorMapSwizzle sw = swizzle == 32 ? CU_TENSOR_MAP_SWIZZLE_32B
+                                : swizzle == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
   CUtensorMap m;
-  CUresult r = enc(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = enc(&m, elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank,
+                   const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    char buf[160];
-    snprintf(buf, sizeof buf, "cuTensorMapEncodeTiled failed (%d) rows=%d cols=%d ld=%lld box=%dx%d", (int)r, rows,
-             cols, ld, box_inner, box_outer);
+    char buf[200];
+    snprintf(buf, sizeof buf, "cuTensorMapEncodeTiled failed (%d) rows=%d cols=%d groups=%d ld=%lld box=%dx%d", (int)r,
+             rows, cols, groups, ld, box_inner, box_outer);
     return ofk_set_error(OFK_ERR_DRIVER, buf);
   }
   {
@@ -605,7 +587,8 @@ static int g_reserved_sms = 0;   // SMs the persistent grids leave free (ofk_gem
 // narrow shape runs.  Cluster slots come from the occupancy of this kernel's shared-memory size, since not every GPC
 // can hold an even number of these CTAs, less the reserved SMs, in whole clusters.
 template <int A_MN, int B_MN, int EPI>
-static int launch(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p, cudaStream_t stream) {
+static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const CUtensorMap& to2,
+                  const CUtensorMap& tx, GemmParams p, cudaStream_t stream) {
   auto kern = gemm_kernel<A_MN, B_MN, EPI>;
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute cluster_attr;
@@ -633,6 +616,10 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p, cu
   const int wide_work = (m_tiles + 1) / 2 * ((p.N + BN_WIDE - 1) / BN_WIDE) * p.splits;
   const int last_split_kb = (p.K + BK - 1) / BK - (p.splits - 1) * p.kb_per_split;   // the shortest split
   p.wide = cluster_slots > 0 && wide_work >= cluster_slots && last_split_kb >= SmemLayout::STAGES;
+  p.m_units = p.wide ? (m_tiles + 1) / 2 : m_tiles;
+  p.n_tiles = (p.N + (p.wide ? BN_WIDE : BN) - 1) / (p.wide ? BN_WIDE : BN);
+  p.num_work = p.m_units * p.n_tiles * p.splits;
+  p.total_kb = (p.K + BK - 1) / BK;
   if (p.wide) {
     cfg.gridDim = dim3(CLUSTER * cluster_slots);
     cfg.attrs = &cluster_attr;
@@ -644,20 +631,49 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p, cu
     cfg.attrs = nullptr;
     cfg.numAttrs = 0;
   }
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, p);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, to, to2, tx, p);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) return ofk_set_error(OFK_ERR_CUDA, cudaGetErrorString(e));
   ofk_count_launch();
   return 0;
 }
 
+// The epilogue's tensor maps, boxes of 64 rows x SUBN columns: out as a 3-D map (columns, rows in group, groups; one
+// group of M rows without a grouped row map), out2 and aux as 2-D maps.  Absent operands get a copy of out's map.
+// A grouped out map's box never crosses a group, so every store is at non-negative coordinates:
+//   rows_per_group % 64 == 0: {SUBN, 64, 1}, one store per 64 rows;
+//   64 % rows_per_group == 0: {SUBN, rpg, 64 / rpg}, 64 / rpg whole groups in one store (decoding: rpg = 1);
+//   otherwise               : {SUBN, h, 1} with h = gcd(rpg, 64), 64 / h stores per 64 rows (group starts are
+//                             multiples of h, and so is every 64-row block).
 template <int EPI>
 static int dispatch_major(int a_mn, int b_mn, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p,
                           cudaStream_t s) {
-  if (a_mn == 0 && b_mn == 0) return launch<0, 0, EPI>(ta, tb, p, s);
-  if (a_mn == 0 && b_mn == 1) return launch<0, 1, EPI>(ta, tb, p, s);
-  if (a_mn == 1 && b_mn == 1) return launch<1, 1, EPI>(ta, tb, p, s);
-  return launch<1, 0, EPI>(ta, tb, p, s);
+  using E = EpiTraits<EPI>;
+  CUtensorMap to, to2, tx;
+  const int ob = E::OUT_BYTES;
+  int rc;
+  if (p.out_rpg > 0) {
+    const int rpg = p.out_rpg;
+    const int box_rows = rpg % 64 == 0 ? 64 : 64 % rpg == 0 ? rpg : p.out_chunk;
+    const int box_groups = rpg % 64 != 0 && 64 % rpg == 0 ? 64 / rpg : 1;
+    rc = get_tensor_map(static_cast<const uint8_t*>(p.out) + (long long)p.out_go * p.ldo * ob, p.ldo, rpg, p.N,
+                        E::SUBN, box_rows, &to, ob, E::OUT_PITCH, p.M / rpg, (long long)p.out_gs * p.ldo, box_groups);
+  } else
+    rc = get_tensor_map(p.out, p.ldo, p.M, p.N, E::SUBN, 64, &to, ob, E::OUT_PITCH, 1, (long long)p.M * p.ldo);
+  if (rc) return rc;
+  to2 = tx = to;
+  if (E::HAS_OUT2 && p.out2 != nullptr) {
+    rc = get_tensor_map(p.out2, p.ldo2, p.M, p.N, E::SUBN, 64, &to2, 2, E::OUT2_PITCH);
+    if (rc) return rc;
+  }
+  if (E::AUX_BYTES != 0) {
+    rc = get_tensor_map(p.aux, p.ldaux, p.M, p.N, E::SUBN, 64, &tx, E::AUX_BYTES, E::SUBN * E::AUX_BYTES);
+    if (rc) return rc;
+  }
+  if (a_mn == 0 && b_mn == 0) return launch<0, 0, EPI>(ta, tb, to, to2, tx, p, s);
+  if (a_mn == 0 && b_mn == 1) return launch<0, 1, EPI>(ta, tb, to, to2, tx, p, s);
+  if (a_mn == 1 && b_mn == 1) return launch<1, 1, EPI>(ta, tb, to, to2, tx, p, s);
+  return launch<1, 0, EPI>(ta, tb, to, to2, tx, p, s);
 }
 
 static int dispatch_epi(int epi, int a_mn, int b_mn, const CUtensorMap& ta, const CUtensorMap& tb,
@@ -687,6 +703,8 @@ static int gemm_impl(int epi, int a_mn_major, int b_mn_major, const void* A, lon
   using namespace ofk;
   if (out_rpg > 0 && (epi != OFK_EPI_STORE_BF16 && epi != OFK_EPI_BIAS_BF16 && epi != OFK_EPI_STORE_F32))
     return ofk_set_error(OFK_ERR_ARG, "grouped output rows are supported by the STORE_BF16 / BIAS_BF16 / STORE_F32 epilogues");
+  if (out_rpg > 0 && M % out_rpg != 0)   // the output map holds whole groups (M / rows_per_group of them)
+    return ofk_set_error(OFK_ERR_ARG, "grouped output rows need M to be a multiple of rows_per_group");
   if (ak_rpg > 0 && (!a_mn_major || ak_rpg % 64 != 0 || K % ak_rpg != 0))
     return ofk_set_error(OFK_ERR_ARG, "grouped reduction rows need an MN-major A with rows_per_group % 64 == 0 dividing K");
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
@@ -703,8 +721,8 @@ static int gemm_impl(int epi, int a_mn_major, int b_mn_major, const void* A, lon
   if ((epi == OFK_EPI_GATE_RESID_F32 || epi == OFK_EPI_BIAS_RESID_F32 || epi == OFK_EPI_DGELU_BF16) && !aux)
     return ofk_set_error(OFK_ERR_ARG, "epilogue needs aux operand");
   if (epi == OFK_EPI_GELU_DUAL && !out2) return ofk_set_error(OFK_ERR_ARG, "GELU_DUAL needs out2");
-  // TMA needs 16-byte-aligned operand bases and row strides; the epilogue moves out / out2 / aux in 16-byte pieces
-  // and reads the bias as float4, so the same holds for every epilogue operand it touches.
+  // TMA needs 16-byte-aligned bases and row strides, for the operands and for the epilogue's out / out2 / aux maps
+  // alike; the bias keeps the 16-byte alignment it has always been checked for.
   auto misaligned = [](const void* ptr, long long ld, int elem_bytes) {
     return (reinterpret_cast<uintptr_t>(ptr) & 15) != 0 || ((ld * elem_bytes) & 15) != 0;
   };
@@ -733,6 +751,11 @@ static int gemm_impl(int epi, int a_mn_major, int b_mn_major, const void* A, lon
   p.splits = (total_kb + p.kb_per_split - 1) / p.kb_per_split;
   p.out = out; p.ldo = ldo; p.out2 = out2; p.ldo2 = ldo2; p.aux = aux; p.ldaux = ldaux; p.bias = bias; p.gate = gate;
   p.out_rpg = out_rpg; p.out_gs = out_gs; p.out_go = out_go; p.ak_rpg = ak_rpg; p.ak_gs = ak_gs; p.ak_go = ak_go;
+  p.out_chunk = 64;   // rows per grouped store (see dispatch_major)
+  if (out_rpg > 0 && out_rpg % 64 != 0 && 64 % out_rpg != 0) {
+    p.out_chunk = 1;
+    while (out_rpg % (2 * p.out_chunk) == 0) p.out_chunk *= 2;   // gcd(rpg, 64): rpg is not a multiple of 64
+  }
   p.wide = 0;   // chosen by launch()
   const int a_rows = ak_rpg > 0 ? (K / ak_rpg) * ak_gs : K;   // physical row count of an MN-major A
   {

@@ -76,6 +76,46 @@ __device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUte
       : "memory");
 }
 
+// Stores shared -> global of one box of a 2-D / 3-D tensor map, tracked as bulk groups of the issuing thread.  Box
+// elements outside the tensor's extents (including negative coordinates) are not written.  `_hint` variants carry an
+// L2 cache policy (createpolicy).
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(m), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void tma_store_2d_hint(const CUtensorMap* m, const void* smem_src, int c0, int c1,
+                                                  uint64_t policy) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3}], [%1], %4;"
+               ::"l"(m), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "l"(policy) : "memory");
+}
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* smem_src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(m), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+__device__ __forceinline__ void tma_store_3d_hint(const CUtensorMap* m, const void* smem_src, int c0, int c1, int c2,
+                                                  uint64_t policy) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3, %4}], [%1], %5;"
+               ::"l"(m), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "l"(policy) : "memory");
+}
+// global[box] += shared[box] (element type of the map; one add per element, performed at L2)
+__device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* m, const void* smem_src, int c0, int c1, int c2) {
+  asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(m), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// All but the newest N bulk groups of this thread have finished reading their shared-memory sources.
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// All bulk groups of this thread are complete (their writes performed).
+__device__ __forceinline__ void bulk_wait_group_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+
 // ---------------------------------------------------------------- thread-block clusters
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;

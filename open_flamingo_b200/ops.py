@@ -594,7 +594,8 @@ def attn_dense_bwd(q, k, v, o, d_o, lse, heads, head_dim, scale, *, causal=False
 def gemm_grouped(a, b, *, a_mn=False, b_mn=False, epi=L.EPI_STORE_BF16, out, M, N, K, bias=None, splits=1, block_n=0,
                  out_map=(0, 0, 0), ak_map=(0, 0, 0)):
     """GEMM with grouped row maps (see ofk_gemm_bf16_grouped): `out_map` = (rows_per_group, group_stride,
-    group_offset) for the rows of `out`; `ak_map` the same for the reduction rows of an MN-major `a`."""
+    group_offset) for the rows of `out`, with M a whole number of groups; `ak_map` the same for the reduction rows of
+    an MN-major `a`."""
     L.require_cuda(a, b, out)
     _rowmajor_2d(a, "a")
     _rowmajor_2d(b, "b")
