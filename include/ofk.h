@@ -359,6 +359,38 @@ int ofk_swiglu_fwd(const void* gu, long long ldgu, int rows, int F, void* h, lon
 int ofk_swiglu_bwd(const void* dh, long long lddh, const void* gu, long long ldgu, int rows, int F, void* dgu,
                    long long lddgu, void* stream);
 
+/* OPT decoder block (HF OPTDecoderLayer, pre-LN, under autocast; modeling_opt.py OPTAttention.forward and
+ * OPTDecoderLayer.forward):
+ * ofk_relu_bf16:      h(bf16) = relu(z(bf16)), n elements, exact (a NaN passes through); h may be z.
+ * ofk_relu_bwd_bf16:  dz(bf16) = h <= 0 ? 0 : dh, from the relu output h (torch's threshold_backward); dz may be dh.
+ *   n % 8 == 0 (OFK_ERR_ARG); every pointer 16-byte aligned (OFK_ERR_ALIGN).
+ * ofk_scale_bf16:     y(bf16) = bf16(x * s) over [rows, cols] (ldx, ldy): OPTAttention's q_proj(x) * scaling on the bf16
+ *   projection, and the same product for its gradient; y may be x.  rows >= 1, cols a positive multiple of 8,
+ *   ldx and ldy >= cols (OFK_ERR_ARG); strides multiples of 8, x and y 16-byte aligned (OFK_ERR_ALIGN).
+ * Every argument is checked before the first CUDA call. */
+int ofk_relu_bf16(const void* z, void* h, long long n, void* stream);
+int ofk_relu_bwd_bf16(const void* dh, const void* h, void* dz, long long n, void* stream);
+int ofk_scale_bf16(const void* x, long long ldx, int rows, int cols, float s, void* y, long long ldy, void* stream);
+
+/* Residual dropout (OPTDecoderLayer: residual + nn.functional.dropout(branch, p) in training, with the branch a bf16
+ * Linear output and the residual the fp32 stream):
+ * ofk_dropout_resid_fwd:  out(f32)[r, c] = kept(r, c) ? x[r, c] + bf16(branch(bf16)[r, c] * scale) : x[r, c]
+ * ofk_dropout_resid_bwd:  dbranch(bf16)[r, c] = kept(r, c) ? bf16(bf16(dout(f32)[r, c]) * scale) : 0
+ *   scale = float(1 / (double)float(1 - p)), torch's dropout scale.  kept(r, c): Philox-4x32-10 with key = seed and
+ *   counter = (c / 4, r, offset low word, offset high word) gives four 32-bit words; word c % 4 >= floor(p * 2^32)
+ *   keeps the element.  seed_offset: device int64 [2] = (seed, offset), read on the device (so a captured graph may
+ *   advance it between replays); may be NULL when p == 0, which keeps everything (out = x + branch, the bits of a
+ *   GATE_RESID_F32 epilogue without gate).  The backward regenerates the forward's mask from the same pair; no mask
+ *   is stored.  out may be x.
+ *   Requirements: x, branch, out (dout, dbranch) non-NULL, p in [0, 1), a seed pair when p > 0, rows >= 1, cols a
+ *   positive multiple of 8, every stride >= cols (OFK_ERR_ARG); f32 strides multiples of 4, bf16 strides multiples
+ *   of 8, seed_offset 8-byte aligned, the other pointers 16-byte aligned (OFK_ERR_ALIGN).  Every argument is checked
+ *   before the first CUDA call. */
+int ofk_dropout_resid_fwd(const float* x, long long ldx, const void* branch, long long ldb, int rows, int cols,
+                          double p, const long long* seed_offset, float* out, long long ldo, void* stream);
+int ofk_dropout_resid_bwd(const float* dout, long long ldd, int rows, int cols, double p,
+                          const long long* seed_offset, void* dbranch, long long lddb, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * CLIP image preprocessing: open_clip's eval transform (image_transform(is_train=False), the image_processor that
  * create_model_and_transforms returns, factory.py:42) on decoded uint8 pixels:

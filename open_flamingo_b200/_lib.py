@@ -15,6 +15,7 @@ c_void_p = ctypes.c_void_p
 c_int = ctypes.c_int
 c_ll = ctypes.c_longlong
 c_float = ctypes.c_float
+c_double = ctypes.c_double
 
 # epilogue ids (include/ofk.h)
 EPI_STORE_BF16 = 0
@@ -83,6 +84,12 @@ _SIGNATURES = {
                                 c_void_p, c_ll, c_void_p]),
     "ofk_swiglu_fwd": (c_int, [c_void_p, c_ll, c_int, c_int, c_void_p, c_ll, c_void_p]),
     "ofk_swiglu_bwd": (c_int, [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_void_p, c_ll, c_void_p]),
+    "ofk_relu_bf16": (c_int, [c_void_p, c_void_p, c_ll, c_void_p]),
+    "ofk_relu_bwd_bf16": (c_int, [c_void_p, c_void_p, c_void_p, c_ll, c_void_p]),
+    "ofk_scale_bf16": (c_int, [c_void_p, c_ll, c_int, c_int, c_float, c_void_p, c_ll, c_void_p]),
+    "ofk_dropout_resid_fwd": (c_int, [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_double, c_void_p, c_void_p, c_ll,
+                                      c_void_p]),
+    "ofk_dropout_resid_bwd": (c_int, [c_void_p, c_ll, c_int, c_int, c_double, c_void_p, c_void_p, c_ll, c_void_p]),
     "ofk_text_time": (c_int, [c_void_p, c_ll, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "ofk_cast_f32_bf16": (c_int, [c_void_p, c_void_p, c_ll, c_void_p]),
     "ofk_reduce_workspace_bytes": (c_ll, []),

@@ -108,6 +108,53 @@ __global__ void gelu_bf16_kernel(const uint4* __restrict__ z, uint4* __restrict_
   }
 }
 
+// ---- OPT's MLP activation and q scaling (HF OPTDecoderLayer under autocast).
+// relu of a bf16 value is exact: h = z > 0 ? z : 0 (a NaN passes through, as torch.relu gives it).  z may be h.
+__device__ __forceinline__ uint32_t relu_bf16x2(uint32_t u) {
+  uint32_t r = u;
+  if ((u & 0x8000u) && (u & 0x7fffu) <= 0x7f80u) r &= 0xffff0000u;           // low half: negative or -0, not NaN
+  if ((u & 0x80000000u) && (u & 0x7fff0000u) <= 0x7f800000u) r &= 0x0000ffffu;
+  return r;
+}
+
+__global__ void relu_bf16_kernel(const uint4* z, uint4* h, long long n8) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += stride) {
+    const uint4 u = z[i];
+    h[i] = make_uint4(relu_bf16x2(u.x), relu_bf16x2(u.y), relu_bf16x2(u.z), relu_bf16x2(u.w));
+  }
+}
+
+// dz = h <= 0 ? 0 : dh with h the relu output (torch's threshold_backward on the result); dz may be dh.
+__device__ __forceinline__ uint32_t relu_bwd_bf16x2(uint32_t d, uint32_t h) {
+  return (bf16_lo(h) <= 0.0f ? 0u : (d & 0xffffu)) | (bf16_hi(h) <= 0.0f ? 0u : (d & 0xffff0000u));
+}
+
+__global__ void relu_bwd_bf16_kernel(const uint4* dh, const uint4* __restrict__ h, uint4* dz, long long n8) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += stride) {
+    const uint4 d = dh[i], v = h[i];
+    dz[i] = make_uint4(relu_bwd_bf16x2(d.x, v.x), relu_bwd_bf16x2(d.y, v.y), relu_bwd_bf16x2(d.z, v.z),
+                       relu_bwd_bf16x2(d.w, v.w));
+  }
+}
+
+// y = bf16(x * s) over a strided [rows, cols] bf16 block (OPTAttention's q_proj(x) * scaling, and its gradient);
+// y may be x.  One 8-column group of one row per item.
+__global__ void scale_bf16_kernel(const __nv_bfloat16* x, long long ldx, int cols, float s, __nv_bfloat16* y,
+                                  long long ldy, long long n8) {
+  const int c8 = cols / 8;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += stride) {
+    const long long r = i / c8;
+    const int c = (int)(i % c8) * 8;
+    const uint4 u = *reinterpret_cast<const uint4*>(x + r * ldx + c);
+    *reinterpret_cast<uint4*>(y + r * ldy + c) =
+        make_uint4(pack_bf16x2(bf16_lo(u.x) * s, bf16_hi(u.x) * s), pack_bf16x2(bf16_lo(u.y) * s, bf16_hi(u.y) * s),
+                   pack_bf16x2(bf16_lo(u.z) * s, bf16_hi(u.z) * s), pack_bf16x2(bf16_lo(u.w) * s, bf16_hi(u.w) * s));
+  }
+}
+
 // ---- SwiGLU of the LLaMA MLP (HF LlamaMLP: act_fn(gate_proj(x)) * up_proj(x)), on the output gu = [g | u] of one
 // GEMM against the concatenated gate|up weight.  silu is torch's x / (1 + exp(-x)) in fp32, rounded to bf16 as
 // autocast rounds act_fn's output; exp(-g) = inf for very negative g gives -0, never NaN.
@@ -365,6 +412,42 @@ extern "C" int ofk_gelu_bf16(const void* z, void* h, long long n, void* stream) 
   if (n % 8 != 0) return ofk_set_error(OFK_ERR_ARG, "gelu: n must be a multiple of 8");
   if (misaligned(z, 16) || misaligned(h, 16)) return ofk_set_error(OFK_ERR_ALIGN, "gelu: pointers must be 16-byte aligned");
   gelu_bf16_kernel<<<grid_for(n / 8, 256), 256, 0, (cudaStream_t)stream>>>((const uint4*)z, (uint4*)h, n / 8);
+  OFK_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int ofk_relu_bf16(const void* z, void* h, long long n, void* stream) {
+  if (!z || !h) return ofk_set_error(OFK_ERR_ARG, "relu: null pointer");
+  if (n <= 0) return 0;
+  if (n % 8 != 0) return ofk_set_error(OFK_ERR_ARG, "relu: n must be a multiple of 8");
+  if (misaligned(z, 16) || misaligned(h, 16)) return ofk_set_error(OFK_ERR_ALIGN, "relu: pointers must be 16-byte aligned");
+  relu_bf16_kernel<<<grid_for(n / 8, 256), 256, 0, (cudaStream_t)stream>>>((const uint4*)z, (uint4*)h, n / 8);
+  OFK_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int ofk_relu_bwd_bf16(const void* dh, const void* h, void* dz, long long n, void* stream) {
+  if (!dh || !h || !dz) return ofk_set_error(OFK_ERR_ARG, "relu bwd: null pointer");
+  if (n <= 0) return 0;
+  if (n % 8 != 0) return ofk_set_error(OFK_ERR_ARG, "relu bwd: n must be a multiple of 8");
+  if (misaligned(dh, 16) || misaligned(h, 16) || misaligned(dz, 16))
+    return ofk_set_error(OFK_ERR_ALIGN, "relu bwd: pointers must be 16-byte aligned");
+  relu_bwd_bf16_kernel<<<grid_for(n / 8, 256), 256, 0, (cudaStream_t)stream>>>((const uint4*)dh, (const uint4*)h,
+                                                                               (uint4*)dz, n / 8);
+  OFK_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int ofk_scale_bf16(const void* x, long long ldx, int rows, int cols, float s, void* y, long long ldy,
+                              void* stream) {
+  if (!x || !y) return ofk_set_error(OFK_ERR_ARG, "scale: null pointer");
+  if (rows < 1 || cols < 1 || cols % 8 != 0 || ldx < cols || ldy < cols)
+    return ofk_set_error(OFK_ERR_ARG, "scale: rows >= 1, cols a positive multiple of 8, ldx and ldy >= cols");
+  if (ldx % 8 != 0 || ldy % 8 != 0) return ofk_set_error(OFK_ERR_ALIGN, "scale: ldx and ldy must be multiples of 8");
+  if (misaligned(x, 16) || misaligned(y, 16)) return ofk_set_error(OFK_ERR_ALIGN, "scale: x and y must be 16-byte aligned");
+  const long long n8 = (long long)rows * (cols / 8);
+  scale_bf16_kernel<<<grid_for(n8, 256), 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)x, ldx, cols, s,
+                                                                          (__nv_bfloat16*)y, ldy, n8);
   OFK_CHECK_LAUNCH();
   return 0;
 }

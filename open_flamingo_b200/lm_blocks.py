@@ -1,6 +1,6 @@
 """Frozen-LM decoder blocks on the sm_90a kernels (SURVEY.md section 8f, rank 1): HF `MptBlock` (OF-3B, OF-9B),
-HF `GPTNeoXLayer` (OF-4B; see the GPT-NeoX section below) and HF `LlamaDecoderLayer` (OF-9B v1; see the LLaMA
-section).
+HF `GPTNeoXLayer` (OF-4B; see the GPT-NeoX section below), HF `LlamaDecoderLayer` (OF-9B v1; see the LLaMA
+section) and HF `OPTDecoderLayer` (see the OPT section).
 
 The reference runs the frozen LM's decoder block as ordinary PyTorch (`self.decoder_layer(lang_x, ...)`,
 flamingo_lm.py:63-65).  For the LM family named by BASELINE.json (MPT: HF `MptBlock` = LN -> Wqkv -> causal
@@ -13,7 +13,7 @@ Decoding with a KV cache runs on the kernels too when the cache is a kv_cache.KV
 (`no_grad` / `inference_mode`): the K/V projection GEMM (GPT-NeoX: the rotary packing) writes the new rows straight
 into the cache buffer, one new token attends through the split-KV decode kernel (ops.attn_decode) and a multi-token
 chunk (prefill, or a chunk after a prefix) through the dense kernel over the cached keys.  Anything else -- other LM
-families, HF's DynamicCache, dropout, clip_qkv, output_attentions (GPT-NeoX: also output_hidden_states, which HF
+families, HF's DynamicCache, dropout (but OPT's residual dropout, see the OPT section), clip_qkv, output_attentions (GPT-NeoX: also output_hidden_states, which HF
 records with hooks on the layer modules) -- takes the block's own PyTorch forward, exactly as in the reference (a
 block that declines still reads and extends a KVCache through HF's attention module and `KVCache.update`).
 
@@ -905,9 +905,319 @@ class FastLlamaBlock:
         return out if out.dtype == hidden_states.dtype else out.to(hidden_states.dtype)
 
 
+# ---- OPT (HF OPTDecoderLayer, pre-LN: OPT-125m, 1.3B, 2.7B, 6.7B) ----------------------------------------------------
+#
+#   a = LN1(x);  q = bf16(bf16(a Wq^T + bq) * s), s = hd^-0.5;  k, v = a Wk^T + bk, a Wv^T + bv
+#   x1 = x + dropout_p(bf16(softmax(q k^T + mask) v Wo^T + bo))          (OPTAttention scales q, attention at scale 1)
+#   out = x1 + dropout_p(bf16(relu(bf16(LN2(x1) W1^T + b1)) W2^T + b2))
+#
+# Q, K and V come from one BIAS_BF16 GEMM against the packed per-head (q | k | v) copy of [Wq; Wk; Wv] (_qkv16, as for
+# LLaMA) and the matching packed bias; ofk_rope_pack without rotation splits the heads (head_dim 80 zero-padded to 128,
+# as for GPT-NeoX) and ofk_scale_bf16 then rounds q * s to bf16, the rounding HF makes (s is exact at head_dim 64 only).
+# The backward applies the same product to dq before ofk_rope_unpack_bwd.
+#
+# The residual dropout (OPT configs set dropout = 0.1, and the frozen LM trains in train mode) runs as a BIAS_BF16 GEMM
+# followed by ofk_dropout_resid_fwd; its backward regenerates the mask from the saved (seed, offset) pair.  With
+# dropout off (eval, or p = 0) the residual adds are BIAS_RESID_F32 epilogues, the same bits in one pass.
+
+
+class _DropoutRng:
+    """Per-device dropout state: `state` = int64 device (seed, next offset).  Each dropout call takes the pair with
+    capturable device ops (a clone, then the offset advanced in place), so a captured training step draws fresh masks
+    at every replay.  The seed is drawn from torch's default CUDA generator; it is drawn again whenever that generator
+    was re-seeded since (its initial seed changed, or its offset went back below where the draw left it), so
+    `torch.manual_seed` reproduces a run.  Re-seeding is checked on eager calls only, never while a graph is captured."""
+
+    def __init__(self, device):
+        self.device = device
+        self.state = torch.zeros(2, dtype=torch.int64, device=device)
+        self.mark = None   # (initial seed, generator offset) right after the last draw
+
+    def _reseed_if_needed(self):
+        gen = torch.cuda.default_generators[self.device.index]
+        if self.mark is not None and gen.initial_seed() == self.mark[0] and gen.get_offset() >= self.mark[1]:
+            return
+        seed = torch.empty(1, dtype=torch.int64, device=self.device).random_(generator=gen)
+        self.state[0:1].copy_(seed)
+        self.state[1:2].zero_()
+        self.mark = (gen.initial_seed(), gen.get_offset())
+
+    def take(self):
+        """A fresh int64 (seed, offset) pair for one dropout call."""
+        if not torch.cuda.is_current_stream_capturing():
+            self._reseed_if_needed()
+        pair = self.state.clone()
+        self.state[1:2].add_(1)
+        return pair
+
+
+_dropout_rngs = {}
+
+
+def dropout_rng(device):
+    """The _DropoutRng of a CUDA device."""
+    device = torch.device(device)
+    if device.index is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    rng = _dropout_rngs.get(device.index)
+    if rng is None:
+        rng = _dropout_rngs[device.index] = _DropoutRng(device)
+    return rng
+
+
+def _qkv_bias(bq, bk, bv, heads):
+    """fp32 [3D] packed bias matching _qkv16's rows: element (h * 3 + p) * hd + j is element h * hd + j of part p."""
+    def fill(ps):
+        D = ps[0].shape[0]
+        t = torch.empty((heads, 3, D // heads), device=ps[0].device, dtype=f32)
+        for i, b in enumerate(ps):
+            t[:, i].copy_(b.detach().view(heads, D // heads))
+        return t.view(3 * D)
+    return _packed_w16(("qkv bias", heads), (bq, bk, bv), fill)
+
+
+def _opt_resid(branch_in, w16_, bias, x2d, p):
+    """x2d + dropout_p(bf16(branch_in W^T + bias)): (sum, the (seed, offset) pair or None when dropout is off)."""
+    if p > 0:
+        so = dropout_rng(x2d.device).take()
+        y = ops.gemm(branch_in, w16_, epi=L.EPI_BIAS_BF16, bias=bias)
+        return ops.dropout_resid_fwd(x2d, y, p, so), so
+    return ops.gemm(branch_in, w16_, epi=L.EPI_BIAS_RESID_F32, bias=bias, aux=x2d), None
+
+
+def _opt_tail(x2d, o, p, eps2, wo16, bo, n2_w, n2_b, w1, b1, w2, b2, want_stats):
+    """The block after its attention core.  x2d: [R, D] f32 block input; o: [R, heads * width] bf16 attention output;
+    wo16: the bf16 out-projection weight for that width; p: the residual dropout probability (0 = off).  Returns
+    (out, x1, mean2, rstd2, h, so1, so2): LayerNorm-2 statistics (None unless want_stats), h = relu(bf16(fc1)) and the
+    two dropout pairs (None when off)."""
+    x1, so1 = _opt_resid(o, wo16, bo, x2d, p)
+    un, mean2, rstd2 = ops.layernorm_fwd(x1, n2_w, n2_b, eps2, want_stats=want_stats)
+    h = ops.gemm(un, w16(w1), epi=L.EPI_BIAS_BF16, bias=b1)
+    del un
+    ops.relu_bf16(h, out=h)
+    out, so2 = _opt_resid(h, w16(w2), b2, x1, p)
+    return out, x1, mean2, rstd2, h, so1, so2
+
+
+def _opt_qkv(xn, B, T, heads, wq, wk, wv, bq, bk, bv):
+    return ops.gemm(xn, _qkv16(wq, wk, wv, heads), epi=L.EPI_BIAS_BF16,
+                    bias=_qkv_bias(bq, bk, bv, heads)).view(B, T, 3 * heads * (wq.shape[0] // heads))
+
+
+class FrozenOptBlockFn(torch.autograd.Function):
+    """A frozen pre-LN OPTDecoderLayer: forward, and the backward to its input only (the parameters take no gradient).
+    x: [B, T, D] f32; mask: [B, T, T] bytes (nonzero = masked) or None for causal only; p: residual dropout (0 = off)."""
+
+    @staticmethod
+    def forward(ctx, x, mask, pure_flag, heads, p, eps1, eps2, n1_w, n1_b, wq, wk, wv, bq, bk, bv, wo, bo, n2_w, n2_b,
+                w1, b1, w2, b2):
+        B, T, D = x.shape
+        R = B * T
+        hd = D // heads
+        W = _neox_width(hd)
+        s = float(hd ** -0.5)
+        x2d = _rows(x)
+        xn, mean1, rstd1 = ops.layernorm_fwd(x2d, n1_w, n1_b, eps1)
+        qkv = _opt_qkv(xn, B, T, heads, wq, wk, wv, bq, bk, bv)
+        del xn
+        q, k, v = ops.rope_pack(qkv, heads, hd, q_width=W, kv_width=W)
+        del qkv
+        ops.scale_bf16(q, s, out=q)
+        o, lse = ops.attn_dense_fwd(q, k, v, heads, W, 1.0, causal=mask is None, mask=mask, pure_causal_flag=pure_flag)
+        out, x1, mean2, rstd2, h, so1, so2 = _opt_tail(x2d, o.view(R, heads * W), p, eps2, _padded_w16(wo, heads, hd, W),
+                                                       bo, n2_w, n2_b, w1, b1, w2, b2, want_stats=True)
+        empty = x2d.new_empty(0)
+        ctx.save_for_backward(x2d, mean1, rstd1, q, k, v, o, lse, x1, mean2, rstd2, h, n1_w, wq, wk, wv, wo, n2_w, w1, w2,
+                              mask if mask is not None else empty, pure_flag if pure_flag is not None else empty,
+                              so1 if so1 is not None else empty, so2 if so2 is not None else empty)
+        ctx.meta = (B, T, D, heads, hd, W, s, p, mask is not None, pure_flag is not None)
+        return out.view(B, T, D)
+
+    @staticmethod
+    def backward(ctx, dout):
+        (x2d, mean1, rstd1, q, k, v, o, lse, x1, mean2, rstd2, h, n1_w, wq, wk, wv, wo, n2_w, w1, w2, mask, pure_flag,
+         so1, so2) = ctx.saved_tensors
+        B, T, D, heads, hd, W, s, p, has_mask, has_flag = ctx.meta
+        mask = mask if has_mask else None
+        pure_flag = pure_flag if has_flag else None
+        R = B * T
+        d2 = _rows(dout)
+        if d2.dtype != f32:
+            d2 = d2.float()
+        dy2 = ops.dropout_resid_bwd(d2, p, so2) if p > 0 else ops.gate_bwd(d2, None, None, None)
+        dh = ops.gemm(dy2, w16(w2), b_mn=True)                                       # [R, F]
+        del dy2
+        ops.relu_bwd_bf16(dh, h, out=dh)
+        du = ops.gemm(dh, w16(w1), b_mn=True)
+        del dh
+        dx1 = ops.layernorm_bwd(du, x1, n2_w, mean2, rstd2, dx_add=d2)
+        del du
+        dy1 = ops.dropout_resid_bwd(dx1, p, so1) if p > 0 else ops.gate_bwd(dx1, None, None, None)
+        d_o = ops.gemm(dy1, _padded_w16(wo, heads, hd, W), b_mn=True)               # [R, heads * W], padding zero
+        del dy1
+        dq, dk, dv = ops.attn_dense_bwd(q, k, v, o, d_o.view(B, T, heads * W), lse, heads, W, 1.0,
+                                        causal=mask is None, mask=mask, pure_causal_flag=pure_flag)
+        del d_o
+        ops.scale_bf16(dq, s, out=dq)                                                 # d(q_proj) = bf16(dq * s)
+        dqkv = ops.rope_unpack_bwd(dq, dk, dv, heads, hd)                             # [B, T, 3D]
+        del dq, dk, dv
+        dxn = ops.gemm(dqkv.view(R, 3 * D), _qkv16(wq, wk, wv, heads), b_mn=True)
+        dx = ops.layernorm_bwd(dxn, x2d, n1_w, mean1, rstd1, dx_add=dx1)
+        return (dx.view(B, T, D),) + (None,) * 22
+
+
+def cached_opt_block_forward(x, layer, mask, pure_flag, heads, p, eps1, eps2, n1_w, n1_b, wq, wk, wv, bq, bk, bv, wo, bo,
+                             n2_w, n2_b, w1, b1, w2, b2):
+    """Inference forward of one OPT block that appends its nq new tokens to `layer` (a kv_cache.KVCacheLayer, unpadded
+    head_dim rows, so HF's attention can extend it through KVCacheLayer.update) and attends over everything cached.
+    ops.rope_pack (no rotation) writes the K and V straight into cache rows [past, past + nq).
+      nq == 1: q unpadded, the decode kernel at head_dim hd, the out-projection with Wo itself;
+      nq > 1 : q and the cached K/V rows [0, nk) padded to the core's width, the dense kernel, the padded Wo.
+    mask: as for cached_block_forward.  x: [B, nq, D] f32; returns the same."""
+    B, nq, D = x.shape
+    hd = D // heads
+    x2d = _rows(x)
+    xn, _, _ = ops.layernorm_fwd(x2d, n1_w, n1_b, eps1, want_stats=False)
+    qkv = _opt_qkv(xn, B, nq, heads, wq, wk, wv, bq, bk, bv)
+    del xn
+    if not layer.is_initialized:
+        layer.init_storage(B, heads, hd, bf16, x.device)
+    past = layer.length
+    rows = layer.reserve(nq)[:, past:past + nq]
+    W = hd if nq == 1 else _neox_width(hd)
+    q, _, _ = ops.rope_pack(qkv, heads, hd, q_width=W, k=rows[..., :D], v=rows[..., D:])
+    del qkv
+    ops.scale_bf16(q, float(hd ** -0.5), out=q)
+    layer.length = past + nq
+    k, v = layer.kv_views()
+    if nq == 1:
+        o = ops.attn_decode(q.view(B, D), k, v, heads, hd, 1.0, key_mask=mask)
+    else:
+        if W != hd:
+            _, k, v = ops.rope_pack(None, heads, hd, kv_src=(k, v), kv_width=W)
+        o, _ = ops.attn_dense_fwd(q, k, v, heads, W, 1.0, causal=mask is None, mask=mask, pure_causal_flag=pure_flag,
+                                  want_lse=False)
+    return _opt_tail(x2d, o.view(B * nq, heads * W), p, eps2, _padded_w16(wo, heads, hd, W), bo, n2_w, n2_b, w1, b1,
+                     w2, b2, want_stats=False)[0].view(B, nq, D)
+
+
+class FastOptBlock:
+    """Callable with HF OPTDecoderLayer.forward's signature; returns None when the fast path does not apply, and the
+    block's output tensor otherwise.
+
+    Graph-replayed decoding does not cover OPT: decode_graph.eligible declines an LM that is neither GPT-NeoX nor has
+    MPT's `transformer` / `norm_f`, so `generate(..., cache_implementation="static")` runs the eager cached path on the
+    fixed-capacity KVCache, step by step, with the bits of a growing KVCache (see FastLlamaBlock)."""
+
+    def __init__(self, block):
+        self.block = block
+
+    def records_outputs(self, output_attentions=None, output_hidden_states=None):
+        """Whether the caller asked HF to record this layer's hidden states or attention weights, which OPTDecoder
+        does with hooks on the modules the fast path does not call (see FastNeoXBlock.records_outputs)."""
+        cfg = self.block.self_attn.config
+        if output_attentions is None:
+            output_attentions = getattr(cfg, "output_attentions", False)
+        if output_hidden_states is None:
+            output_hidden_states = getattr(cfg, "output_hidden_states", False)
+        return bool(output_attentions or output_hidden_states)
+
+    def supported(self, hidden_states, record_outputs):
+        """The block and call are ones the kernels evaluate, whatever the cache."""
+        b = self.block
+        a = b.self_attn
+        if not ENABLED or not hidden_states.is_cuda or record_outputs:
+            return False
+        if not b.do_layer_norm_before or getattr(a.config, "activation_function", None) != "relu":
+            return False   # post-LN (OPT-350m) and other activations are HF's
+        hd = a.head_dim
+        if hd not in (64, 80, 128) or abs(a.scaling - hd ** -0.5) > 1e-9 or a.embed_dim != a.num_heads * hd:
+            return False
+        if a.embed_dim > 4096 or b.fc1.out_features % 16:
+            return False   # the LayerNorm kernels take D <= 4096; the fc2 dgrad GEMM has N = ffn_dim
+        if b.training and a.dropout > 0:
+            return False   # attention-probability dropout is not in the attention cores
+        if not 0.0 <= self.dropout_p() < 1.0:
+            return False
+        lins = (a.q_proj, a.k_proj, a.v_proj, a.out_proj, b.fc1, b.fc2)
+        norms = (b.self_attn_layer_norm, b.final_layer_norm)
+        if any(m.bias is None for m in lins) or any(n.weight is None or n.bias is None for n in norms):
+            return False
+        if any(p.dtype != f32 for p in b.parameters()):
+            return False
+        if any(p.requires_grad for p in b.parameters()):
+            return False   # this path has no wgrad: frozen blocks only
+        return True
+
+    def dropout_p(self):
+        """The residual dropout probability this call applies: the layer's in training mode, else 0."""
+        return float(self.block.dropout) if self.block.training else 0.0
+
+    def weights(self):
+        b = self.block
+        a = b.self_attn
+        return (b.self_attn_layer_norm.weight, b.self_attn_layer_norm.bias, a.q_proj.weight, a.k_proj.weight,
+                a.v_proj.weight, a.q_proj.bias, a.k_proj.bias, a.v_proj.bias, a.out_proj.weight, a.out_proj.bias,
+                b.final_layer_norm.weight, b.final_layer_norm.bias, b.fc1.weight, b.fc1.bias, b.fc2.weight, b.fc2.bias)
+
+    def step_args(self):
+        """The head count, dropout probability and LayerNorm eps of the block, then its weights: the arguments after
+        pure_flag of FrozenOptBlockFn and cached_opt_block_forward."""
+        b = self.block
+        return (b.self_attn.num_heads, self.dropout_p(), b.self_attn_layer_norm.eps,
+                b.final_layer_norm.eps) + self.weights()
+
+    def applicable(self, hidden_states, past_key_values, use_cache, record_outputs):
+        """The uncached path (FrozenOptBlockFn, forward and backward)."""
+        if past_key_values is not None or use_cache:
+            return False
+        return self.supported(hidden_states, record_outputs)
+
+    def cache_layer(self, hidden_states, past_key_values, record_outputs):
+        """The KVCacheLayer the cached path appends to, or None (see FastMptBlock.cache_layer)."""
+        if not isinstance(past_key_values, KVCache) or torch.is_grad_enabled():
+            return None
+        if not self.supported(hidden_states, record_outputs):
+            return None
+        a = self.block.self_attn
+        if a.layer_idx is None or not 0 <= a.layer_idx < len(past_key_values.layers):
+            return None
+        layer = past_key_values.layers[a.layer_idx]
+        if layer.is_initialized and (layer.buf.dtype != bf16 or layer.buf.device != hidden_states.device or
+                                     layer.buf.shape[0] != hidden_states.shape[0] or
+                                     layer.heads != a.num_heads or layer.head_dim != a.head_dim):
+            return None
+        return layer
+
+    def __call__(self, hidden_states, attention_mask=None, past_key_values=None, use_cache=False, position_ids=None,
+                 output_attentions=None, output_hidden_states=None, pure_causal_flag=None, **kwargs):
+        record = self.records_outputs(output_attentions, output_hidden_states)
+        layer = None
+        if past_key_values is not None or use_cache:
+            layer = self.cache_layer(hidden_states, past_key_values, record)
+            if layer is None:
+                return None
+        elif not self.applicable(hidden_states, past_key_values, use_cache, record):
+            return None
+        B, T, _ = hidden_states.shape
+        nk = T if layer is None else layer.length + T
+        mask = None
+        if attention_mask is not None:   # HF's sdpa mask, True = attend; a float (eager) mask is declined here
+            mask = _kernel_mask(attention_mask, B, T, nk, layer is not None and T == 1, true_attends=True)
+            if mask is None:
+                return None
+        x = hidden_states if hidden_states.dtype == f32 else hidden_states.float()
+        flag = pure_causal_flag if mask is not None else None
+        if layer is not None:
+            out = cached_opt_block_forward(x, layer, mask, flag, *self.step_args())
+        else:
+            out = FrozenOptBlockFn.apply(x, mask, flag, *self.step_args())
+        return out if out.dtype == hidden_states.dtype else out.to(hidden_states.dtype)
+
+
 def accelerate(decoder_layer):
-    """Return a fast evaluator for a recognised frozen decoder block (HF MptBlock, GPTNeoXLayer or LlamaDecoderLayer),
-    else None."""
+    """Return a fast evaluator for a recognised frozen decoder block (HF MptBlock, GPTNeoXLayer, LlamaDecoderLayer or
+    OPTDecoderLayer), else None."""
     name = type(decoder_layer).__name__
     if name == "MptBlock" and hasattr(decoder_layer, "attn") and hasattr(decoder_layer, "ffn"):
         return FastMptBlock(decoder_layer)
@@ -915,4 +1225,6 @@ def accelerate(decoder_layer):
         return FastNeoXBlock(decoder_layer)
     if name == "LlamaDecoderLayer" and hasattr(decoder_layer, "self_attn") and hasattr(decoder_layer, "mlp"):
         return FastLlamaBlock(decoder_layer)
+    if name == "OPTDecoderLayer" and hasattr(decoder_layer, "self_attn") and hasattr(decoder_layer, "fc1"):
+        return FastOptBlock(decoder_layer)
     return None

@@ -880,3 +880,98 @@ def clip_preprocess(images, size, mean, std, *, out=None):
     L.check(lib.ofk_clip_preprocess(plan.data_ptr(), plan_bytes.value, ws.data_ptr(), ws_bytes.value, out.data_ptr(),
                                     out.stride(0) if n > 1 else 3 * S * S, L.stream_ptr()))
     return out
+
+
+def relu_bf16(z, out=None):
+    """h = relu(z) for a contiguous bf16 z (ofk_relu_bf16), exact; `out` may be z itself."""
+    L.require_cuda(z, out)
+    _vector(z, "z", bf16, z.numel())
+    if out is None:
+        out = torch.empty(z.shape, device=z.device, dtype=bf16)
+    _vector(out, "out", bf16, z.numel())
+    L.check(L.lib().ofk_relu_bf16(z.data_ptr(), out.data_ptr(), z.numel(), L.stream_ptr()))
+    return out
+
+
+def relu_bwd_bf16(dh, h, out=None):
+    """dz = dh where the relu output h > 0, else 0 (ofk_relu_bwd_bf16); contiguous bf16 of one size, `out` may be dh."""
+    L.require_cuda(dh, h, out)
+    _vector(dh, "dh", bf16, dh.numel())
+    _vector(h, "h", bf16, dh.numel())
+    if out is None:
+        out = torch.empty(dh.shape, device=dh.device, dtype=bf16)
+    _vector(out, "out", bf16, dh.numel())
+    L.check(L.lib().ofk_relu_bwd_bf16(dh.data_ptr(), h.data_ptr(), out.data_ptr(), dh.numel(), L.stream_ptr()))
+    return out
+
+
+def scale_bf16(x, s, out=None):
+    """y = bf16(x * s) (ofk_scale_bf16) over the rows of x: bf16, 2-D or 3-D with unit inner stride and rows at one
+    stride (e.g. [B, T, C] contiguous, or a column slice).  `out` (same shape, allocated when None) may be x."""
+    L.require_cuda(x, out)
+    if x.dtype != bf16 or x.dim() not in (2, 3) or x.stride(-1) != 1 or \
+            (x.dim() == 3 and x.shape[0] > 1 and x.stride(0) != x.shape[1] * x.stride(1)):
+        raise ValueError(f"x must be a bf16 [rows, C] or [B, T, C] view with unit inner stride and evenly spaced rows, "
+                         f"got {tuple(x.shape)} {x.dtype} stride {x.stride()}")
+    if out is None:
+        out = torch.empty(x.shape, device=x.device, dtype=bf16)
+    if out.dtype != bf16 or out.shape != x.shape or out.stride(-1) != 1 or \
+            (out.dim() == 3 and out.shape[0] > 1 and out.stride(0) != out.shape[1] * out.stride(1)):
+        raise ValueError(f"out must be a bf16 view of shape {tuple(x.shape)} with unit inner stride and evenly spaced "
+                         f"rows, got {tuple(out.shape)} {out.dtype} stride {out.stride()}")
+    cols = x.shape[-1]
+    rows = x.numel() // cols if cols else 0
+    if rows:
+        L.check(L.lib().ofk_scale_bf16(x.data_ptr(), x.stride(-2), rows, cols, float(s), out.data_ptr(), out.stride(-2),
+                                       L.stream_ptr()))
+    return out
+
+
+def _seed_offset(seed_offset, p):
+    if p > 0 and (seed_offset is None or seed_offset.dtype != torch.int64 or seed_offset.numel() != 2 or
+                  not seed_offset.is_contiguous()):
+        raise ValueError("dropout with p > 0 needs seed_offset, a contiguous int64 device tensor (seed, offset)")
+
+
+def dropout_resid_fwd(x, branch, p, seed_offset, out=None):
+    """out = x + dropout_p(branch) (ofk_dropout_resid_fwd): x [rows, C] f32, branch [rows, C] bf16, both with unit inner
+    stride; p in [0, 1); seed_offset: int64 device (seed, offset) (unused, may be None, at p = 0).  Returns out [rows, C]
+    f32 (`out`, allocated when None; may be x)."""
+    L.require_cuda(x, branch, seed_offset, out)
+    _rowmajor_2d(x, "x")
+    _rowmajor_2d(branch, "branch")
+    if x.dtype != f32 or branch.dtype != bf16 or branch.shape != x.shape:
+        raise ValueError(f"x must be float32 and branch bfloat16 of one shape, got {tuple(x.shape)} {x.dtype} and "
+                         f"{tuple(branch.shape)} {branch.dtype}")
+    _seed_offset(seed_offset, p)
+    if out is None:
+        out = torch.empty(x.shape, device=x.device, dtype=f32)
+    _rowmajor_2d(out, "out")
+    if out.dtype != f32 or out.shape != x.shape:
+        raise ValueError(f"out must be float32 of shape {tuple(x.shape)}")
+    rows, cols = x.shape
+    if rows:
+        L.check(L.lib().ofk_dropout_resid_fwd(x.data_ptr(), x.stride(0), branch.data_ptr(), branch.stride(0), rows, cols,
+                                              float(p), L.ptr(seed_offset), out.data_ptr(), out.stride(0),
+                                              L.stream_ptr()))
+    return out
+
+
+def dropout_resid_bwd(dout, p, seed_offset, out=None):
+    """Gradient of dropout_resid_fwd's branch (ofk_dropout_resid_bwd): dout [rows, C] f32 with unit inner stride ->
+    dbranch [rows, C] bf16 (`out`, allocated when None), from the forward's p and seed_offset."""
+    L.require_cuda(dout, seed_offset, out)
+    _rowmajor_2d(dout, "dout")
+    if dout.dtype != f32:
+        raise ValueError("dout must be float32")
+    _seed_offset(seed_offset, p)
+    if out is None:
+        out = torch.empty(dout.shape, device=dout.device, dtype=bf16)
+    _rowmajor_2d(out, "out")
+    if out.dtype != bf16 or out.shape != dout.shape:
+        raise ValueError(f"out must be bfloat16 of shape {tuple(dout.shape)}")
+    rows, cols = dout.shape
+    if rows:
+        L.check(L.lib().ofk_dropout_resid_bwd(dout.data_ptr(), dout.stride(0), rows, cols, float(p),
+                                              L.ptr(seed_offset), out.data_ptr(), out.stride(0), L.stream_ptr()))
+    return out

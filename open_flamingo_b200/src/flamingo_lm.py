@@ -32,7 +32,7 @@ class FlamingoLayer(nn.Module):
         self.vis_x = None
         self.media_locations = None
         self.use_cached_media = None
-        # recognised frozen decoder blocks (HF MptBlock, GPTNeoXLayer, LlamaDecoderLayer) are evaluated on the sm_90a
+        # recognised frozen decoder blocks (HF MptBlock, GPTNeoXLayer, LlamaDecoderLayer, OPTDecoderLayer) run on the sm_90a
         # kernels; everything else -- and every case the fast path declines -- runs the block's own PyTorch forward as
         # in the reference
         self._fast_block = lm_blocks.accelerate(decoder_layer)
@@ -163,12 +163,22 @@ class FlamingoLMMixin(nn.Module):
             if attention_mask is not None:
                 m4 = m4 | (attention_mask == 0).view(input_ids.shape[0], 1, 1, T)
             attention_mask = m4.contiguous()
+        elif input_ids.is_cuda and torch.cuda.is_current_stream_capturing() and \
+                type(self).__mro__[2].__name__.startswith("OPT") and attention_mask is not None and \
+                attention_mask.dim() == 2 and kwargs.get("past_key_values") is None and kwargs.get("position_ids") is None:
+            # The same for OPT, whose decoder also derives its learned positions from the 2-D mask: hand it those
+            # positions (OPTDecoder's own formula) and the 4-D mask in its sdpa form, True = attend =
+            # (key not after query) & (key is not padding).
+            B, T = input_ids.shape
+            kwargs["position_ids"] = (torch.cumsum(attention_mask, dim=1) * attention_mask - 1).long()
+            causal = torch.ones(T, T, dtype=torch.bool, device=input_ids.device).tril()
+            attention_mask = (causal.view(1, 1, T, T) & (attention_mask != 0).view(B, 1, 1, T)).contiguous()
         return super().forward(input_ids=input_ids, attention_mask=attention_mask, **kwargs)
 
     def make_kv_cache(self, capacity=None):
         """A kv_cache.KVCache for decoding this LM on the kernels, or None where HF's own cache is kept: it is made only
         on CUDA, under `torch.autocast("cuda", dtype=torch.bfloat16)` (the caller asked for bf16 numerics; the cache
-        stores bf16), with lm_blocks.ENABLED, and when every decoder block is a recognised MPT, GPT-NeoX or LLaMA block.  In
+        stores bf16), with lm_blocks.ENABLED, and when every decoder block is a recognised MPT, GPT-NeoX, LLaMA or OPT block.  In
         fp32 every path stays HF's.
 
         capacity: None for a cache that grows; an int for a fixed-capacity cache of at least that many rows, with which

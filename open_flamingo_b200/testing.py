@@ -95,12 +95,31 @@ def build_llama(llama_kw, dtype=torch.float32, device="cpu", seed=0):
     return lm.to(dtype).eval()
 
 
+# OPT-1.3B (facebook/opt-1.3b): D 2048, 32 heads of 64, 24 layers, FFN 8192; OPT-2.7B: D 2560, 32 heads of 80, 32 layers,
+# FFN 10240.  Both pre-LN with ReLU, biases and residual dropout 0.1, as the released configs set them.
+OPT_1_3B = dict(hidden_size=2048, num_attention_heads=32, num_hidden_layers=24, ffn_dim=8192, vocab_size=50272,
+                max_position_embeddings=2048, word_embed_proj_dim=2048, dropout=0.1, attention_dropout=0.0,
+                activation_function="relu", do_layer_norm_before=True)
+OPT_2_7B = dict(OPT_1_3B, hidden_size=2560, num_hidden_layers=32, ffn_dim=10240, word_embed_proj_dim=2560)
+
+
+def build_opt(opt_kw, dtype=torch.float32, device="cpu", seed=0):
+    """Random-init HF OPTForCausalLM from an OPTConfig (offline), attention through sdpa, whose boolean mask is what the
+    kernels take."""
+    from transformers import OPTConfig, OPTForCausalLM
+    torch.manual_seed(seed)
+    cfg = OPTConfig(**opt_kw, attn_implementation="sdpa")
+    with torch.device(device):
+        lm = OPTForCausalLM(cfg)
+    return lm.to(dtype).eval()
+
+
 def build_flamingo(vit_cfg, mpt_kw, cross_attn_every_n_layers=1, device="cuda", freeze_lm_embeddings=True, seed=0,
-                   lm_dtype=torch.float32, gate_init=None, neox_kw=None, llama_kw=None):
+                   lm_dtype=torch.float32, gate_init=None, neox_kw=None, llama_kw=None, opt_kw=None):
     """Random-init Flamingo through the public factory.  gate_init: None keeps the reference's zero gates
     (helpers.py:255,258); a float f draws gates ~ U(-f, f) so the gated path is actually exercised.  neox_kw: build
     the LM with build_neox(neox_kw) instead of an MPT from mpt_kw (pass mpt_kw=None); llama_kw likewise with
-    build_llama."""
+    build_llama, opt_kw with build_opt."""
     torch.manual_seed(seed)
     with torch.device(device):
         vit = VisionTransformer(**vit_cfg)
@@ -110,6 +129,9 @@ def build_flamingo(vit_cfg, mpt_kw, cross_attn_every_n_layers=1, device="cuda", 
     elif llama_kw is not None:
         lm = build_llama(llama_kw, dtype=lm_dtype, device=device, seed=seed + 1)
         base_vocab = llama_kw["vocab_size"]
+    elif opt_kw is not None:
+        lm = build_opt(opt_kw, dtype=lm_dtype, device=device, seed=seed + 1)
+        base_vocab = opt_kw["vocab_size"]
     else:
         lm = build_mpt(mpt_kw, dtype=lm_dtype, device=device, seed=seed + 1)
         base_vocab = mpt_kw["vocab_size"]
