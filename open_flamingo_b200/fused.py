@@ -60,6 +60,29 @@ def w16(param):
     return t
 
 
+_wpad_cache = {}
+
+
+def padded_w16(param, heads, hd, width):
+    """bf16 copy of an out-projection weight [D, heads * hd] with each head's columns zero-padded to `width`:
+    [D, heads * width].  It lets the out-projection read an attention output whose heads were run zero-padded on the
+    head_dim-128 cores (GPT-NeoX and OPT at head_dim 80, ViT-H/g/bigG).  Refreshed by w16's rule -- a weakly referenced
+    parameter at the same version counter and address -- so `load_state_dict` or an in-place edit is seen."""
+    if width == hd:
+        return w16(param)
+    key = id(param)
+    ent = _wpad_cache.get(key)
+    if ent is not None and ent[0]() is param and ent[1] == param._version and ent[2] == param.data_ptr():
+        return ent[3]
+    D = param.shape[0]
+    t = torch.zeros((D, heads, width), device=param.device, dtype=bf16)
+    t[..., :hd].copy_(w16(param).view(D, heads, hd))   # a layout change of the bf16 copy, made once per weight version
+    t = t.view(D, heads * width)
+    _wpad_cache[key] = (weakref.ref(param, lambda _r, k=key: _wpad_cache.pop(k, None)), param._version,
+                        param.data_ptr(), t)
+    return t
+
+
 class _GradSink:
     """Where a parameter's gradient goes: its `_ofk_grad` bucket view (accumulate, return None) or a fresh tensor."""
 

@@ -26,7 +26,7 @@ import torch
 
 from . import _lib as L
 from . import ops
-from .fused import w16
+from .fused import padded_w16, w16
 from .kv_cache import KVCache
 
 bf16 = torch.bfloat16
@@ -325,7 +325,7 @@ class FastMptBlock:
 # on the 128 cores with every head zero-padded to 128 columns: ops.rope_pack writes the rotated q, k and v in that
 # layout, zero columns add exact zeros to q k^T, to P v and to every backward product, so the result is the head_dim-80
 # attention.  The attention output then has H * 128 columns; the out-projection reads it through a copy of Wd with the
-# same zero columns (_padded_w16), and in the backward the dgrad GEMM with that copy yields the padded d_o directly.
+# same zero columns (fused.padded_w16), and in the backward the dgrad GEMM with that copy yields the padded d_o directly.
 # Decoding one token runs the decode kernel at head_dim 80 directly, on an unpadded KV cache; its graph-captured form
 # (decode_step_neox_block_forward) writes the new K/V row with ops.rope_append_dev at a position read on the device.
 
@@ -333,28 +333,6 @@ class FastMptBlock:
 def _neox_width(hd):
     """Head width the attention cores run a head_dim-hd head at."""
     return hd if hd in (64, 128) else 128
-
-
-_wpad_cache = {}
-
-
-def _padded_w16(param, heads, hd, width):
-    """bf16 copy of an out-projection weight [D, heads * hd] with each head's columns zero-padded to `width`:
-    [D, heads * width].  Refreshed by w16's rule -- a weakly referenced parameter at the same version counter and
-    address -- so `load_state_dict` or an in-place edit is seen."""
-    if width == hd:
-        return w16(param)
-    key = id(param)
-    ent = _wpad_cache.get(key)
-    if ent is not None and ent[0]() is param and ent[1] == param._version and ent[2] == param.data_ptr():
-        return ent[3]
-    D = param.shape[0]
-    t = torch.zeros((D, heads, width), device=param.device, dtype=bf16)
-    t[..., :hd].copy_(w16(param).view(D, heads, hd))   # a layout change of the bf16 copy, made once per weight version
-    t = t.view(D, heads * width)
-    _wpad_cache[key] = (weakref.ref(param, lambda _r, k=key: _wpad_cache.pop(k, None)), param._version,
-                        param.data_ptr(), t)
-    return t
 
 
 def _neox_tail(x2d, o, parallel, eps2, wout16, bd, n2_w, n2_b, w1, b1, w2, b2, keep_z):
@@ -403,7 +381,7 @@ class FrozenNeoXBlockFn(torch.autograd.Function):
         scale = float(hd ** -0.5)
         o, lse = ops.attn_dense_fwd(q, k, v, heads, W, scale, causal=mask is None, mask=mask,
                                     pure_causal_flag=pure_flag)
-        out, x1, mean2, rstd2, z = _neox_tail(x2d, o.view(R, heads * W), parallel, eps2, _padded_w16(wd, heads, hd, W),
+        out, x1, mean2, rstd2, z = _neox_tail(x2d, o.view(R, heads * W), parallel, eps2, padded_w16(wd, heads, hd, W),
                                               bd, n2_w, n2_b, w1, b1, w2, b2, keep_z=True)
         ctx.save_for_backward(x2d, mean1, rstd1, q, k, v, o, lse, x1, mean2, rstd2, z, cos, sin, n1_w, wqkv, wd, n2_w,
                               w1, w2, mask if mask is not None else x2d.new_empty(0),
@@ -430,7 +408,7 @@ class FrozenNeoXBlockFn(torch.autograd.Function):
         dx1 = ops.layernorm_bwd(du, x2d if parallel else x1, n2_w, mean2, rstd2, dx_add=d2)
         del du
         dy = dbr if parallel else ops.gate_bwd(dx1, None, None, None)
-        d_o = ops.gemm(dy, _padded_w16(wd, heads, hd, W), b_mn=True)                # [R, heads * W], padding zero
+        d_o = ops.gemm(dy, padded_w16(wd, heads, hd, W), b_mn=True)                 # [R, heads * W], padding zero
         del dy, dbr
         dq, dk, dv = ops.attn_dense_bwd(q, k, v, o, d_o.view(B, T, heads * W), lse, heads, W, scale,
                                         causal=mask is None, mask=mask, pure_causal_flag=pure_flag)
@@ -473,7 +451,7 @@ def cached_neox_block_forward(x, layer, mask, pure_flag, cos, sin, heads, parall
             _, k, v = ops.rope_pack(None, heads, hd, kv_src=(k, v), kv_width=W)
         o, _ = ops.attn_dense_fwd(q, k, v, heads, W, scale, causal=mask is None, mask=mask, pure_causal_flag=pure_flag,
                                   want_lse=False)
-    return _neox_tail(x2d, o.view(B * nq, heads * W), parallel, eps2, _padded_w16(wd, heads, hd, W), bd, n2_w, n2_b,
+    return _neox_tail(x2d, o.view(B * nq, heads * W), parallel, eps2, padded_w16(wd, heads, hd, W), bd, n2_w, n2_b,
                       w1, b1, w2, b2, keep_z=False)[0].view(B, nq, D)
 
 
@@ -1024,7 +1002,7 @@ class FrozenOptBlockFn(torch.autograd.Function):
         del qkv
         ops.scale_bf16(q, s, out=q)
         o, lse = ops.attn_dense_fwd(q, k, v, heads, W, 1.0, causal=mask is None, mask=mask, pure_causal_flag=pure_flag)
-        out, x1, mean2, rstd2, h, so1, so2 = _opt_tail(x2d, o.view(R, heads * W), p, eps2, _padded_w16(wo, heads, hd, W),
+        out, x1, mean2, rstd2, h, so1, so2 = _opt_tail(x2d, o.view(R, heads * W), p, eps2, padded_w16(wo, heads, hd, W),
                                                        bo, n2_w, n2_b, w1, b1, w2, b2, want_stats=True)
         empty = x2d.new_empty(0)
         ctx.save_for_backward(x2d, mean1, rstd1, q, k, v, o, lse, x1, mean2, rstd2, h, n1_w, wq, wk, wv, wo, n2_w, w1, w2,
@@ -1053,7 +1031,7 @@ class FrozenOptBlockFn(torch.autograd.Function):
         dx1 = ops.layernorm_bwd(du, x1, n2_w, mean2, rstd2, dx_add=d2)
         del du
         dy1 = ops.dropout_resid_bwd(dx1, p, so1) if p > 0 else ops.gate_bwd(dx1, None, None, None)
-        d_o = ops.gemm(dy1, _padded_w16(wo, heads, hd, W), b_mn=True)               # [R, heads * W], padding zero
+        d_o = ops.gemm(dy1, padded_w16(wo, heads, hd, W), b_mn=True)                # [R, heads * W], padding zero
         del dy1
         dq, dk, dv = ops.attn_dense_bwd(q, k, v, o, d_o.view(B, T, heads * W), lse, heads, W, 1.0,
                                         causal=mask is None, mask=mask, pure_causal_flag=pure_flag)
@@ -1097,7 +1075,7 @@ def cached_opt_block_forward(x, layer, mask, pure_flag, heads, p, eps1, eps2, n1
             _, k, v = ops.rope_pack(None, heads, hd, kv_src=(k, v), kv_width=W)
         o, _ = ops.attn_dense_fwd(q, k, v, heads, W, 1.0, causal=mask is None, mask=mask, pure_causal_flag=pure_flag,
                                   want_lse=False)
-    return _opt_tail(x2d, o.view(B * nq, heads * W), p, eps2, _padded_w16(wo, heads, hd, W), bo, n2_w, n2_b, w1, b1,
+    return _opt_tail(x2d, o.view(B * nq, heads * W), p, eps2, padded_w16(wo, heads, hd, W), bo, n2_w, n2_b, w1, b1,
                      w2, b2, want_stats=False)[0].view(B, nq, D)
 
 

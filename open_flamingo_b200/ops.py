@@ -631,14 +631,15 @@ def _rope_dest(t, name, B, rows, inner):
 
 
 def rope_pack(src, heads, head_dim, cos=None, sin=None, *, q=None, k=None, v=None, q_width=None, kv_width=None,
-              kv_src=None):
+              kv_src=None, blocks=False):
     """Rotary q/k packing of GPT-NeoX rows (ofk_rope_pack).
 
     src: [B, T, heads * 3 * head_dim] bf16 view of the query_key_value output (heads interleaved as (q | k | v)), or
     None with kv_src = (k_rows, v_rows): two [B, T, heads * head_dim] views (the K and V columns of a KV cache) whose
-    heads are only re-laid out.  cos/sin: fp32 [1 or B, T, rot] (None: no rotation).  q / k / v: destinations
-    [B, T, heads * width] (allocated when None and wanted); q_width, kv_width: head widths (default head_dim), columns
-    past head_dim are zero.  Returns (q, k, v); q is None with kv_src."""
+    heads are only re-laid out.  blocks=True: src holds q, k and v as three column blocks of heads * head_dim each
+    (nn.MultiheadAttention's in_proj output, as in the CLIP ViT).  cos/sin: fp32 [1 or B, T, rot] (None: no rotation).
+    q / k / v: destinations [B, T, heads * width] (allocated when None and wanted); q_width, kv_width: head widths
+    (default head_dim), columns past head_dim are zero.  Returns (q, k, v); q is None with kv_src."""
     L.require_cuda(src, cos, sin, q, k, v, *(kv_src or ()))
     q_width = head_dim if q_width is None else q_width
     kv_width = head_dim if kv_width is None else kv_width
@@ -647,9 +648,12 @@ def rope_pack(src, heads, head_dim, cos=None, sin=None, *, q=None, k=None, v=Non
             raise ValueError(f"src must be a bf16 [B, T, {heads * 3 * head_dim}] view with unit inner stride, got "
                              f"{tuple(src.shape)} {src.dtype}")
         B, T = src.shape[:2]
-        srcs = (src, src[..., head_dim:], src[..., 2 * head_dim:])
-        sbs, sld, shs = src.stride(0), src.stride(1), 3 * head_dim
+        part = heads * head_dim if blocks else head_dim   # column offset of k's (and v's) head 0 after q's
+        srcs = (src, src[..., part:], src[..., 2 * part:])
+        sbs, sld, shs = src.stride(0), src.stride(1), head_dim if blocks else 3 * head_dim
     else:
+        if blocks:
+            raise ValueError("rope_pack: blocks=True describes src; it does not apply to kv_src")
         ks, vs = kv_src
         if ks.dtype != bf16 or ks.dim() != 3 or ks.shape != vs.shape or ks.stride() != vs.stride() or \
                 ks.shape[2] != heads * head_dim or ks.stride(2) != 1:

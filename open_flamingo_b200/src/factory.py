@@ -25,6 +25,13 @@ _OPEN_CLIP_VISION_CFG = {
     "ViT-L-14-336": dict(image_size=336, patch_size=14, width=1024, layers=24, heads=16, output_dim=768),
     "ViT-B-16": dict(image_size=224, patch_size=16, width=768, layers=12, heads=12, output_dim=512),
     "ViT-B-32": dict(image_size=224, patch_size=32, width=768, layers=12, heads=12, output_dim=512),
+    # the LaION towers: head widths 80, 88 and 104 (zero-padded heads, see vit.py), exact GELU
+    "ViT-H-14": dict(image_size=224, patch_size=14, width=1280, layers=32, heads=16, output_dim=1024,
+                     quick_gelu=False),
+    "ViT-g-14": dict(image_size=224, patch_size=14, width=1408, layers=40, heads=16, mlp_ratio=4.3637,
+                     output_dim=1024, quick_gelu=False),
+    "ViT-bigG-14": dict(image_size=224, patch_size=14, width=1664, layers=48, heads=16, mlp_ratio=4.9231,
+                        output_dim=1280, quick_gelu=False),
 }
 
 # decoder ModuleList attribute per LM family (reference factory.py:132-141)
@@ -84,9 +91,6 @@ def _build_vision(clip_vision_encoder_path, clip_vision_encoder_pretrained, cach
             name, pretrained=clip_vision_encoder_pretrained, cache_dir=cache_dir)
         cfg = dict(open_clip.get_model_config(name)["vision_cfg"])
         head_width = cfg.get("head_width", 64)
-        if head_width != 64:
-            raise ValueError(f"{name}: head_width {head_width} (open_clip vision_cfg) is not supported -- the sm_90a "
-                             "ViT attention kernel is built for head_dim 64 (ViT-B/L; ViT-H/g/bigG use 80-104)")
         ours = VisionTransformer(image_size=cfg.get("image_size", 224), patch_size=cfg["patch_size"],
                                  width=cfg["width"], layers=cfg["layers"], heads=cfg["width"] // head_width,
                                  mlp_ratio=cfg.get("mlp_ratio", 4.0), output_dim=ref_model.visual.proj.shape[1],

@@ -11,6 +11,11 @@ this restates its published VisionTransformer algorithm:
        (patch tokens WITHOUT ln_post -- open_clip 2.16-2.20 behaviour, which is what Flamingo was trained with).
 Parameter names follow open_clip's `visual.*` state dict so pretrained CLIP weights load unchanged.
 Forward only (Flamingo never back-propagates into the ViT, flamingo.py:194).
+
+Head width 64 (ViT-B, ViT-L) runs the media attention core on the in_proj output's q/k/v column blocks.  Other head
+widths (ViT-H 80, ViT-g 88, ViT-bigG 104: any multiple of 8 in (64, 128]) have no core of their own: ops.rope_pack
+copies each head into 128 zero-padded columns, the head_dim-128 dense core runs non-causal and unmasked on them, and
+out_proj reads the padded output through fused.padded_w16 -- the path the GPT-NeoX blocks take at head_dim 80.
 """
 import math
 
@@ -19,7 +24,7 @@ from torch import nn
 
 from .. import _lib as L
 from .. import ops
-from ..fused import w16
+from ..fused import padded_w16, w16
 
 bf16 = torch.bfloat16
 
@@ -60,8 +65,11 @@ class VisionTransformer(nn.Module):
     def __init__(self, image_size=224, patch_size=14, width=1024, layers=24, heads=16, mlp_ratio=4.0,
                  output_dim=768, quick_gelu=True, output_tokens=False):
         super().__init__()
-        if width % heads != 0 or width // heads != 64:
-            raise ValueError("the sm_90a attention kernel needs head_dim == 64 (CLIP ViT-B / ViT-L; not ViT-H/g/bigG)")
+        hd = width // heads if heads > 0 and width % heads == 0 else None
+        if hd is None or not (hd == 64 or (64 < hd <= 128 and hd % 8 == 0)):
+            raise ValueError(f"width {width} over {heads} heads: the sm_90a attention supports head widths 64 "
+                             "(ViT-B, ViT-L) and multiples of 8 in (64, 128] on zero-padded heads (ViT-H 80, ViT-g 88, "
+                             "ViT-bigG 104)")
         self.image_size, self.patch_size, self.width, self.heads = image_size, patch_size, width, heads
         self.grid = image_size // patch_size
         self.output_dim = output_dim
@@ -109,13 +117,24 @@ class VisionTransformer(nn.Module):
         tok = ops.vit_assemble(pe, self.class_embedding, self.positional_embedding, N, g, D)   # fp32 [N*S, D]
         xs, _, _ = ops.layernorm_fwd(tok, self.ln_pre.weight, self.ln_pre.bias, out_f32=True, want_stats=False)
         act = L.EPI_BIAS_QGELU_BF16 if self.quick_gelu else L.EPI_BIAS_GELU_BF16
-        scale = 1.0 / math.sqrt(D // self.heads)
+        heads = self.heads
+        hd = D // heads
+        scale = 1.0 / math.sqrt(hd)
         for blk in self.transformer.resblocks:
             h, _, _ = ops.layernorm_fwd(xs, blk.ln_1.weight, blk.ln_1.bias, want_stats=False)
             qkv = ops.gemm(h, w16(blk.attn.in_proj_weight), epi=L.EPI_BIAS_BF16, bias=blk.attn.in_proj_bias)
             qkv3 = qkv.view(N, S, 3 * D)
-            o, _ = ops.attn_fwd(qkv3[..., :D], qkv3[..., D:2 * D], qkv3[..., 2 * D:], self.heads, scale, want_lse=False)
-            ops.gemm(o.view(N * S, D), w16(blk.attn.out_proj.weight), epi=L.EPI_BIAS_RESID_F32,
+            if hd == 64:
+                o, _ = ops.attn_fwd(qkv3[..., :D], qkv3[..., D:2 * D], qkv3[..., 2 * D:], heads, scale,
+                                    want_lse=False)
+                wo = w16(blk.attn.out_proj.weight)
+            else:
+                # no core at this head_dim: every head zero-padded to 128 columns runs the head_dim-128 dense core,
+                # whose zero columns add exact zeros, and out_proj reads the padded output through zero weight columns
+                q, k, v = ops.rope_pack(qkv3, heads, hd, q_width=128, kv_width=128, blocks=True)
+                o, _ = ops.attn_dense_fwd(q, k, v, heads, 128, scale, causal=False, mask=None, want_lse=False)
+                wo = padded_w16(blk.attn.out_proj.weight, heads, hd, 128)
+            ops.gemm(o.view(N * S, o.shape[-1]), wo, epi=L.EPI_BIAS_RESID_F32,
                      bias=blk.attn.out_proj.bias, aux=xs, out=xs)                   # x += out_proj(attn)  (in place)
             h, _, _ = ops.layernorm_fwd(xs, blk.ln_2.weight, blk.ln_2.bias, want_stats=False)
             f = ops.gemm(h, w16(blk.mlp.c_fc.weight), epi=act, bias=blk.mlp.c_fc.bias)

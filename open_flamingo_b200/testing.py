@@ -2,7 +2,7 @@
 with the OF-3B / OF-9B shapes.  Used by tests, __graft_entry__.smoke() and bench.py."""
 import torch
 
-from .src.factory import create_model_and_transforms
+from .src.factory import _OPEN_CLIP_VISION_CFG, create_model_and_transforms
 from .src.vit import CLIPVisionStandIn, VisionTransformer
 
 
@@ -40,6 +40,12 @@ class SimpleTokenizer:
     def __len__(self):
         return self.base_vocab + len(self.special)
 
+
+# The LaION vision towers wider than ViT-L/14 (open_clip ViT-H-14, ViT-g-14, ViT-bigG-14: head widths 80, 88 and 104),
+# as VisionTransformer keyword arguments for build_flamingo.
+VIT_H14 = dict(_OPEN_CLIP_VISION_CFG["ViT-H-14"])
+VIT_G14 = dict(_OPEN_CLIP_VISION_CFG["ViT-g-14"])
+VIT_BIGG14 = dict(_OPEN_CLIP_VISION_CFG["ViT-bigG-14"])
 
 MPT_1B = dict(d_model=2048, n_heads=16, n_layers=24, vocab_size=50277, max_seq_len=2048, expansion_ratio=4)
 MPT_7B = dict(d_model=4096, n_heads=32, n_layers=32, vocab_size=50277, max_seq_len=2048, expansion_ratio=4)
